@@ -4,8 +4,9 @@
 // Replaces VariableBaseMSM::msm_unchecked for Projective<P> (ec/src/scalar_mul/variable_base/mod.rs:59-64
 // -> msm_bigint_wnaf_parallel :437-503).  Same mathematics, GPU schedule:
 //   reference (per window, serial over points)          here (all windows at once)
-//   into_bigint + make_digits (:60-62, :754-794)    ->  msm_digits_kernel<HIST>: REDC + signed digits, histogram of (window, |digit|)
-//   buckets[|d|-1] +=/-= base  (:467-475)           ->  exclusive scan; msm_digits_kernel<SCATTER> writes (index | sign) in bucket order;
+//   into_bigint + make_digits (:60-62, :754-794)    ->  msm_digits_kernel: REDC + signed digits of every window, written once
+//   buckets[|d|-1] +=/-= base  (:467-475)           ->  msm_sort.cu: two-pass counting sort (coarse bins, then each bin in shared
+//                                                       memory) into (index | sign) in bucket order;
 //                                                       msm_pair_add_kernel x up to 4 levels: every bucket run is halved with AFFINE
 //                                                       additions that share one inversion per batch (Montgomery's trick);
 //                                                       msm_accumulate_kernel: one thread per task of T entries runs the reference's
@@ -358,7 +359,7 @@ template <class C> struct MsmSession final : MsmSessionBase {
     EventSet events;
     std::vector<cudaEvent_t> chunk_ev;   // 5 per chunk
     cudaEvent_t e_begin = nullptr, e_acc_done = nullptr, e_red = nullptr, e_end = nullptr;
-    uint32_t *counts = nullptr, *offsets = nullptr, *cursor = nullptr, *sorted = nullptr, *block_totals = nullptr;
+    uint32_t *counts = nullptr, *offsets = nullptr, *sorted = nullptr, *block_totals = nullptr;
     uint32_t *buckets = nullptr, *extra = nullptr;
     size_t scan_blocks = 0;
     int restore_l2_gran = -1;
@@ -396,7 +397,6 @@ template <class C> struct MsmSession final : MsmSessionBase {
         scan_blocks = (nb_total + kScanBlock - 1) / kScanBlock;
         if (int rc = arena.alloc(&counts, nb_total * 4)) return rc;
         if (int rc = arena.alloc(&offsets, (nb_total + 1) * 4)) return rc;
-        if (int rc = arena.alloc(&cursor, nb_total * 4)) return rc;
         if (int rc = arena.alloc(&sorted, std::max<size_t>(max_entries, 1) * 4)) return rc;
         if (int rc = arena.alloc(&block_totals, std::max<size_t>(scan_blocks, 1) * 4)) return rc;
         if (int rc = arena.alloc(&buckets, nb_total * 4 * L * 4)) return rc;
@@ -528,34 +528,41 @@ template <class C> struct MsmSession final : MsmSessionBase {
         }
         if (nb_total == 0) nk = 0;   // slice without buckets (a window with fewer buckets than slices goes whole to slice 0)
         AB_CUDA(cudaEventRecord(e[0], st));
-        AB_CUDA(cudaMemsetAsync(counts, 0, nb_total * 4, st));
-        if (nk)
-            if (int rc = MsmAccLaunch<C>::digits(0, d_scalars, kind, nk, g, 0, g.W, counts, nullptr, st)) return rc;
-        AB_CUDA(cudaEventRecord(e[1], st));
-        if (nb_total)
-            if (int rc = scan(counts, nb_total, offsets)) return rc;
-        AB_CUDA(cudaMemcpyAsync(cursor, offsets, nb_total * 4, cudaMemcpyDeviceToDevice, st));
-        // entries of the chunk up to each window boundary: the bound nk per window, or — for a bucket slice, which receives only
-        // ~1/slices of it — the counts themselves (one small read-back per chunk; the launch geometry of the levels depends on it)
-        std::vector<size_t> upto((size_t)g.W + 1);
+        // bucket sort: digits (+ group counts) | bin plan | partition + bin sort.  Its scratch is released before the affine
+        // levels, whose budget is taken from the free memory
+        std::vector<size_t> upto((size_t)g.W + 1);   // entries of the chunk up to each window boundary
         for (int w = 0; w <= g.W; w++) upto[w] = nk * (size_t)w;
-        if (sliced && nk) {
-            std::vector<uint32_t> h((size_t)g.W + 1, 0u);
-            for (int w = 1; w <= g.W; w++)
-                AB_CUDA(cudaMemcpyAsync(&h[w], offsets + (w == g.W ? nb_total : (size_t)w * g.nb), 4, cudaMemcpyDeviceToHost, st));
-            AB_CUDA(cudaStreamSynchronize(st));
-            for (int w = 0; w <= g.W; w++) upto[w] = h[w];
+        uint32_t *digits = nullptr, *plan_mem = nullptr;
+        uint2 *part = nullptr;
+        MsmSortPlan plan;
+        if (nk) {
+            if (int rc = arena.alloc(&digits, nk * (size_t)g.W * 4)) return rc;
+            if (int rc = arena.alloc(&plan_mem, MsmSortPlan::bytes(g.W))) return rc;
+            plan.carve(plan_mem, g.W);
+            AB_CUDA(cudaMemsetAsync(plan.gcount, 0, (size_t)g.W * kSortGroups * 4, st));
+            if (int rc = MsmAccLaunch<C>::digits(d_scalars, kind, nk, g, digits, st)) return rc;
+            if (int rc = msm_sort_count(digits, nk, g, plan, st)) return rc;
+        }
+        AB_CUDA(cudaEventRecord(e[1], st));
+        if (nk) {
+            if (int rc = msm_sort_plan(g, plan, offsets, st)) return rc;
+            // a bucket slice receives only ~1/slices of the bound nk per window: its window bases are read back (the launch
+            // geometry of the levels depends on them)
+            if (sliced) {
+                std::vector<uint32_t> h((size_t)g.W + 1, 0u);
+                AB_CUDA(cudaMemcpyAsync(h.data(), plan.wbase, ((size_t)g.W + 1) * 4, cudaMemcpyDeviceToHost, st));
+                AB_CUDA(cudaStreamSynchronize(st));
+                for (int w = 0; w <= g.W; w++) upto[w] = h[w];
+            }
         }
         const size_t entries = upto[g.W];
         AB_CUDA(cudaEventRecord(e[2], st));
-        // scatter in groups of windows so that the active write fronts (one 32-byte sector per bucket of the group) stay
-        // L2-resident: random 4-byte stores into a multi-GB array otherwise cost a DRAM sector each.  The fronts of a group take
-        // at most 16 MB, a third of the H100's 50 MB L2, which also holds the digits being read and the bucket cursors
         if (nk) {
-            const size_t front_bytes = std::max<size_t>(g.nb, 1) * 32;
-            const int group = (int)std::max<size_t>(1, ((size_t)16 << 20) / front_bytes);
-            for (int w0 = 0; w0 < g.W; w0 += group)
-                if (int rc = MsmAccLaunch<C>::digits(1, d_scalars, kind, nk, g, w0, std::min(g.W, w0 + group), cursor, sorted, st)) return rc;
+            if (int rc = arena.alloc(&part, nk * sizeof(uint2))) return rc;
+            if (int rc = msm_sort_scatter(digits, nk, g, plan, part, offsets, sorted, st)) return rc;
+            arena.release(part);
+            arena.release(plan_mem);
+            arena.release(digits);
         }
         AB_CUDA(cudaEventRecord(e[3], st));
         AB_CUDA(cudaMemsetAsync(target, 0, nb_total * 4 * L * 4, st));

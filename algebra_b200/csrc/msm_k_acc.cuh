@@ -1,15 +1,16 @@
-// msm_k_acc.cuh — digit extraction / scatter, task-balanced XYZZ accumulation, fix-ups, bucket merge, and their launchers.
+// msm_k_acc.cuh — digit extraction, task-balanced XYZZ accumulation, fix-ups, bucket merge, and their launchers.
 #pragma once
 #include "msm_common.cuh"
 
 namespace ab200 {
 
 // ------------------------------------------------------------------------------------------------
-// digits: canonical scalar -> signed digits (make_digits, :754-794); MODE 0 = histogram, 1 = scatter
+// digits: canonical scalar -> signed digits (make_digits, :754-794), every window's digit written once, window-major:
+// digits[w * n + i] = rel | sign << 31 (rel = bucket inside the window's slice) or kNoDigit — the input of the bucket sort
 // ------------------------------------------------------------------------------------------------
-template <class C, int MODE>
-__global__ void __launch_bounds__(256) msm_digits_kernel(const void *__restrict__ scalars_v, int kind, size_t n, MsmGeom g, int w_lo, int w_hi,
-                                                         uint32_t *__restrict__ counts_or_cursor, uint32_t *__restrict__ sorted) {
+template <class C>
+__global__ void __launch_bounds__(256) msm_digits_kernel(const void *__restrict__ scalars_v, int kind, size_t n, MsmGeom g,
+                                                         uint32_t *__restrict__ digits) {
     using FR = Fp<typename C::Fr>;
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -44,7 +45,7 @@ __global__ void __launch_bounds__(256) msm_digits_kernel(const void *__restrict_
     const int c = g.c;
     const uint32_t mask = (1u << c) - 1, half = 1u << (c - 1);
     uint32_t carry = 0;
-    for (int w = 0; w < w_hi; w++) {  // the carry chain needs every lower window; only [w_lo, w_hi) is emitted
+    for (int w = 0; w < g.W; w++) {
         const int bit = w * c, wi = bit >> 5, sh = bit & 31;
         uint64_t two = ((uint64_t)k[wi + 1] << 32) | k[wi];
         uint32_t coef = ((uint32_t)(two >> sh) & mask) + carry;
@@ -58,15 +59,8 @@ __global__ void __launch_bounds__(256) msm_digits_kernel(const void *__restrict_
         }
         // bucket slice: only the magnitudes in [off, off + nbw) of each window belong to this session (whole window by default)
         const uint32_t rel = mag - 1 - ((w == g.W - 1) ? g.off_top : g.off);
-        if (mag && w >= w_lo && rel < ((w == g.W - 1) ? g.nb_top : g.nb)) {
-            uint32_t gid = (uint32_t)w * g.nb + rel;
-            if (MODE == 0) {
-                atomicAdd(&counts_or_cursor[gid], 1u);
-            } else {
-                uint32_t pos = atomicAdd(&counts_or_cursor[gid], 1u);
-                sorted[pos] = (uint32_t)i | ((neg ^ flip) << 31);
-            }
-        }
+        const bool keep = mag && rel < ((w == g.W - 1) ? g.nb_top : g.nb);
+        digits[(size_t)w * n + i] = keep ? rel | ((neg ^ flip) << 31) : kNoDigit;
     }
 }
 // ------------------------------------------------------------------------------------------------
@@ -236,12 +230,8 @@ __global__ void __launch_bounds__(128) msm_merge_kernel(uint32_t *__restrict__ b
 }
 
 
-template <class C>
-int MsmAccLaunch<C>::digits(int mode, const void *scalars, int kind, size_t nk, MsmGeom g, int w0, int w1, uint32_t *counts_or_cursor, uint32_t *sorted,
-                            cudaStream_t st) {
-    const unsigned dblocks = (unsigned)((nk + 255) / 256);
-    if (mode == 0) msm_digits_kernel<C, 0><<<dblocks, 256, 0, st>>>(scalars, kind, nk, g, w0, w1, counts_or_cursor, nullptr);
-    else msm_digits_kernel<C, 1><<<dblocks, 256, 0, st>>>(scalars, kind, nk, g, w0, w1, counts_or_cursor, sorted);
+template <class C> int MsmAccLaunch<C>::digits(const void *scalars, int kind, size_t nk, MsmGeom g, uint32_t *digits, cudaStream_t st) {
+    msm_digits_kernel<C><<<(unsigned)((nk + 255) / 256), 256, 0, st>>>(scalars, kind, nk, g, digits);
     AB_LAUNCHED();
     return 0;
 }
