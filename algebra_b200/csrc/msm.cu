@@ -7,14 +7,15 @@
 //   into_bigint + make_digits (:60-62, :754-794)    ->  msm_digits_kernel: REDC + signed digits of every window, written once
 //   buckets[|d|-1] +=/-= base  (:467-475)           ->  msm_sort.cu: two-pass counting sort (coarse bins, then each bin in shared
 //                                                       memory) into (index | sign) in bucket order;
-//                                                       msm_pair_add_kernel x up to 4 levels: every bucket run is halved with AFFINE
-//                                                       additions that share one inversion per batch (Montgomery's trick);
+//                                                       msm_pairmap_kernel + msm_pair_add_kernel x up to 4 levels: every bucket run
+//                                                       is halved with AFFINE additions that share one inversion per block
+//                                                       (Montgomery's trick);
 //                                                       msm_accumulate_kernel: one thread per task of T entries runs the reference's
 //                                                       `Bucket += Affine` (bucket.rs:168-238) on what is left, flushing per bucket;
 //                                                       msm_fixup_*: buckets that span tasks
 //   running-sum  res += running_sum (:478-484)      ->  msm_bucket_reduce_kernel (running sum per chunk of 32 buckets + chunk offset times
 //                                                       chunk total) and msm_sum_partials_kernel (tree over the chunks of a window)
-//   window combine, c doublings per window (:489-502) -> msm_window_combine_kernel (Jacobian, one thread)
+//   window combine, c doublings per window (:489-502) -> msm_window_combine_coop_kernel (Jacobian, one warp)
 // EC addition is commutative/associative, so bucket order, atomics, pairing and chunking do not change the group element;
 // results are compared with the reference after into_affine(), limb-exact.
 // The digit recoding is the reference's make_digits (top window unsigned), so bucket counts per window are 2^(c-1), and
@@ -106,10 +107,10 @@ __global__ void __launch_bounds__(kScanThreads) scan_apply_kernel(const uint32_t
 // ------------------------------------------------------------------------------------------------
 // Batched-affine pre-reduction (optional stage between the sort and the XYZZ accumulation).
 // One level halves every bucket's run: output slot j of bucket b = in[2j] + in[2j+1] (or in[2j] alone when the run is odd),
-// as AFFINE points.  Affine addition needs 1/(x2 - x1); a thread owns `batch` consecutive output slots and inverts all
-// their denominators with ONE field inversion (Montgomery's trick: forward pass stores the running products in the
-// output slots themselves, backward pass peels them off) — ~6 modmuls + inversion/batch per addition instead of the
-// 10 of an XYZZ mixed addition.  Degenerate pairs keep the batch intact with a denominator of 1: an identity operand passes
+// as AFFINE points.  Affine addition needs 1/(x2 - x1); a thread owns `batch` output slots and the 128 threads of a block
+// invert all their denominators with ONE field inversion (Montgomery's trick: forward pass stores the running products in
+// the output slots themselves, backward pass peels them off) — ~6 modmuls + inversion/(128 batch) per addition instead of
+// the 10 of an XYZZ mixed addition.  Degenerate pairs keep the batch intact with a denominator of 1: an identity operand passes
 // the other one through, equal points are doubled (denominator 2y), opposite points give the identity (0,0).
 // Same group element as the reference's bucket sums (EC addition is associative); parity is checked after into_affine().
 // ------------------------------------------------------------------------------------------------
@@ -120,6 +121,9 @@ __global__ void __launch_bounds__(256) msm_halve_counts_kernel(const uint32_t *_
     uint32_t cnt = offsets_in[b + 1] - offsets_in[b];
     counts_out[b] = (cnt + 1) >> 1;
 }
+// pairmap[p] = (index of the first input entry of output slot p) | (the slot has a second entry) << 31.
+// One block per 1024 consecutive slots: two threads locate the first and last bucket of the block's slot range, the bucket
+// offsets in between are staged in shared memory and every slot finds its bucket by a short binary search there (any bucket
 // size distribution costs the same; a run of > 2048 buckets inside one block — mostly empty ones — falls back to global loads).
 __global__ void __launch_bounds__(256) msm_pairmap_kernel(const uint32_t *__restrict__ offsets_in, const uint32_t *__restrict__ offsets_out,
                                                           uint32_t nb, uint32_t *__restrict__ pairmap) {
@@ -166,41 +170,24 @@ __global__ void __launch_bounds__(256) msm_pairmap_kernel(const uint32_t *__rest
 // Options of a call.  Defaults come from the per-thread setters (b200_set_msm_window / _affine_levels) and, for the tuning
 // knobs without a public setter, from environment variables read ONCE per process (never on the call path).
 struct EnvKnobs {
-    int pair_variant = 2;                 // levels >= 2: 1 = thread-contiguous batches, 2 = warp-interleaved + cp.async staging
-    int pair_variant_l1 = 2;              // level 1 (random gathers from the bases): generation 2 stages points with cp.async.ca, so
-                                          // chunks 2..6 of a point hit the L1 line the first chunk brought in
     double level_budget_bytes = 48e9;     // scratch allowed for the affine level arrays (window groups are sized to fit); also capped
                                           // by 60 % of the free device memory at the start of the call, which on an 80 GB H100 is the
                                           // binding limit for 2^26 inputs (the levels of all windows would take ~63 GB).  Fewer groups
                                           // are faster: groups shorten the batches of the later levels
-    int shared_inv = 1;                   // one field inversion per block (Montgomery's trick across the block) instead of per thread
-    int min_batch = 256;                  // automatic mode: shortest per-thread batch a level may run with
-    int target_waves = 1;                 // a level is cut into at least this many waves of resident blocks (when batches stay >= wave_min_batch)
-    int wave_min_batch = 192;
+    int min_batch = 96;                   // automatic mode: shortest per-thread batch a level may run with (overhead per addition:
+                                          // 590/(4*batch) multiplications of the block-shared inversion)
     double level_min_load = 16.0;         // automatic mode: keep adding affine levels while the average bucket still holds this many entries
     int level_cap = 8;                    // upper bound on top of the per-curve LEVEL_CAP
-    int pad_bases = 0;                    // level 1 gathers from a copy of the bases padded to one 128-byte line per point (BLS12-381 G1)
-    int stagger = 0;                      // generation-2 pair-add: unequal batches inside groups of four blocks (desynchronises the inversions)
     int reduce_log_m = 6;                 // buckets per reduction thread = 2^reduce_log_m at most
     bool reduce_log_m_forced = false;     // set through the environment: used as given (tuning runs)
     int force_chunks = 0;                 // test hook: split device-resident inputs into this many chunks
-    int l2_fetch_granularity = 0;         // cudaLimitMaxL2FetchGranularity during the MSM (0 = leave alone)
     EnvKnobs() {
-        if (const char *e = getenv("B200_MSM_PAIR_VARIANT")) pair_variant = atoi(e) == 1 ? 1 : 2;
-        if (const char *e = getenv("B200_MSM_PAIR_VARIANT_L1")) pair_variant_l1 = atoi(e) == 1 ? 1 : 2;
         if (const char *e = getenv("B200_MSM_LEVEL_BUDGET_GB")) { double v = atof(e); if (v > 0.01) level_budget_bytes = v * 1e9; }
-        if (const char *e = getenv("B200_MSM_SHARED_INV")) shared_inv = atoi(e) != 0;
-        min_batch = shared_inv ? 96 : 256;   // overhead per addition: 590/(4*batch) multiplications shared, 570/batch per thread
         if (const char *e = getenv("B200_MSM_MIN_BATCH")) min_batch = std::max(8, atoi(e));
-        if (const char *e = getenv("B200_MSM_TARGET_WAVES")) target_waves = std::max(1, atoi(e));
-        if (const char *e = getenv("B200_MSM_WAVE_MIN_BATCH")) wave_min_batch = std::max(8, atoi(e));
         if (const char *e = getenv("B200_MSM_LEVEL_MIN_LOAD")) level_min_load = std::max(2.0, atof(e));
         if (const char *e = getenv("B200_MSM_LEVEL_CAP")) level_cap = std::min(8, std::max(0, atoi(e)));
-        if (const char *e = getenv("B200_MSM_STAGGER")) stagger = atoi(e) != 0;
-        if (const char *e = getenv("B200_MSM_PAD_BASES")) pad_bases = atoi(e) != 0;
         if (const char *e = getenv("B200_MSM_REDUCE_LOG_M")) { reduce_log_m = std::min(8, std::max(0, atoi(e))); reduce_log_m_forced = true; }
         if (const char *e = getenv("B200_MSM_FORCE_CHUNKS")) force_chunks = atoi(e);
-        if (const char *e = getenv("B200_L2_FETCH_GRANULARITY")) l2_fetch_granularity = atoi(e);
     }
 };
 static const EnvKnobs &env_knobs() {
@@ -362,14 +349,9 @@ template <class C> struct MsmSession final : MsmSessionBase {
     uint32_t *counts = nullptr, *offsets = nullptr, *sorted = nullptr, *block_totals = nullptr;
     uint32_t *buckets = nullptr, *extra = nullptr;
     size_t scan_blocks = 0;
-    int restore_l2_gran = -1;
     bool sliced = false;   // bucket slice of a larger MSM: entry counts are read back per chunk (they are ~1/slices of the bound)
 
     int coord_words() const override { return L; }
-
-    ~MsmSession() override {
-        if (restore_l2_gran >= 0) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)restore_l2_gran);
-    }
 
     int begin(size_t n_total, size_t max_chunk_, int kind_, cudaStream_t st_) override {
         st = st_;
@@ -387,13 +369,6 @@ template <class C> struct MsmSession final : MsmSessionBase {
         const size_t nb_total = g.total_buckets;
         const size_t max_entries = max_chunk * (size_t)g.W;
         if (max_entries >= ((size_t)1 << 31)) { set_last_error("chunk pairs * windows must be < 2^31"); return B200_ETOOLARGE; }
-        if (env_knobs().l2_fetch_granularity > 0) {
-            size_t cur = 0;
-            if (cudaDeviceGetLimit(&cur, cudaLimitMaxL2FetchGranularity) == cudaSuccess) {
-                restore_l2_gran = (int)cur;
-                cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)env_knobs().l2_fetch_granularity);
-            }
-        }
         scan_blocks = (nb_total + kScanBlock - 1) / kScanBlock;
         if (int rc = arena.alloc(&counts, nb_total * 4)) return rc;
         if (int rc = arena.alloc(&offsets, (nb_total + 1) * 4)) return rc;
@@ -451,7 +426,7 @@ template <class C> struct MsmSession final : MsmSessionBase {
     }
 
     // batched-affine levels + XYZZ accumulation of the buckets [b0, b1) (a group of whole windows) of the current chunk
-    int reduce_group(const uint32_t *bas, const uint32_t *bas_padded, size_t b0, size_t b1, size_t group_entries, int levels, uint32_t *target) {
+    int reduce_group(const uint32_t *bas, size_t b0, size_t b1, size_t group_entries, int levels, uint32_t *target) {
         const size_t nbg = b1 - b0;
         const bool forced = levels_opt >= 0;
         size_t cur_entries = group_entries;   // upper bound on the entries of the current level
@@ -462,17 +437,13 @@ template <class C> struct MsmSession final : MsmSessionBase {
         for (int lv = 0; lv < levels; lv++) {
             // sum_b ceil(cnt_b / 2) <= min((entries + non-empty buckets) / 2, entries)
             const size_t out_cap = std::min((cur_entries + nbg) / 2 + 1, cur_entries);
-            // one inversion (~570 modmuls) per `batch` additions.  The grid is sized to a whole number of waves of resident
-            // threads so that no SM idles through a partial last wave; in automatic mode a level that cannot give every
-            // resident thread >= 256 slots is left to the XYZZ kernel instead (measured: thin levels are slower).
+            // one block-shared inversion (~590 modmuls) per 128 `batch` additions.  The grid is sized to a whole number of waves
+            // of resident threads so that no SM idles through a partial last wave; in automatic mode a level that cannot give
+            // every resident thread >= min_batch slots is left to the XYZZ kernel instead (measured: thin levels are slower).
             const double per_lane = (double)out_cap / lanes_per_wave;
             const double min_batch = (double)env_knobs().min_batch;
             if (!forced && per_lane < min_batch) break;
-            double waves = std::max(1.0, std::ceil(per_lane / 1024.0));
-            // a single wave runs every block through the same phase (gather, multiply, invert) at the same time; several shorter
-            // waves let the memory-bound and the arithmetic phases of different blocks overlap
-            if ((double)env_knobs().target_waves > waves)
-                waves = std::max(waves, std::min((double)env_knobs().target_waves, std::floor(per_lane / (double)env_knobs().wave_min_batch)));
+            const double waves = std::max(1.0, std::ceil(per_lane / 1024.0));
             uint32_t batch = (uint32_t)std::ceil((double)out_cap / (waves * lanes_per_wave));
             batch = std::min(1024u, std::max(forced ? 8u : (uint32_t)min_batch, batch));
             uint32_t *pts = nullptr, *off2 = nullptr;
@@ -481,17 +452,11 @@ template <class C> struct MsmSession final : MsmSessionBase {
             msm_halve_counts_kernel<<<(unsigned)((nbg + 255) / 256), 256, 0, st>>>(cur_offsets, (uint32_t)nbg, counts);
             AB_LAUNCHED();
             if (int rc = scan(counts, nbg, off2)) return rc;
-            const int variant = lv == 0 ? env_knobs().pair_variant_l1 : env_knobs().pair_variant;
             uint32_t *pairmap = nullptr;
-            if (variant == 2) {
-                if (int rc = arena.alloc(&pairmap, out_cap * 4)) return rc;
-                msm_pairmap_kernel<<<(unsigned)((out_cap + 1023) / 1024), 256, 0, st>>>(cur_offsets, off2, (uint32_t)nbg, pairmap);
-                AB_LAUNCHED();
-            }
-            const bool padded = lv == 0 && variant == 2 && bas_padded;
-            if (int rc = MsmPairLaunch<C>::run(variant, lv == 0, padded ? bas_padded : bas, cur_src, cur_offsets, off2, pairmap, (uint32_t)nbg, batch, out_cap, pts,
-                                               env_knobs().shared_inv, (variant == 2 && env_knobs().shared_inv) ? env_knobs().stagger : 0, padded ? 32u : 0u, st))
-                return rc;
+            if (int rc = arena.alloc(&pairmap, out_cap * 4)) return rc;
+            msm_pairmap_kernel<<<(unsigned)((out_cap + 1023) / 1024), 256, 0, st>>>(cur_offsets, off2, (uint32_t)nbg, pairmap);
+            AB_LAUNCHED();
+            if (int rc = MsmPairLaunch<C>::run(lv == 0, bas, cur_src, off2, pairmap, (uint32_t)nbg, batch, out_cap, pts, st)) return rc;
             arena.release(pairmap);
             // the level before the previous one is no longer read
             arena.release(lvl_pts[lv & 1]);
@@ -573,7 +538,7 @@ template <class C> struct MsmSession final : MsmSessionBase {
                 levels = 0;
                 if (C::AUTO_LEVELS)
                     for (double l = (double)nk / (double)(1u << (g.c - 1)); l >= env_knobs().level_min_load && levels < std::min(env_knobs().level_cap, C::LEVEL_CAP); l *= 0.5) levels++;
-                // the first level must be able to give every resident thread a batch of >= 256 additions
+                // the first level must be able to give every resident thread a batch of >= min_batch additions
                 if ((double)entries * 0.5 / ((double)sm_count() * C::PAIR_MINB * 128.0) < (double)env_knobs().min_batch) levels = 0;
             }
             if (levels == 0) {
@@ -593,17 +558,11 @@ template <class C> struct MsmSession final : MsmSessionBase {
                 gw = std::min(g.W, gw);
                 const int ngroups = (g.W + gw - 1) / gw;
                 gw = (g.W + ngroups - 1) / ngroups;
-                uint32_t *bas_padded = nullptr;
-                if (env_knobs().pad_bases && env_knobs().pair_variant_l1 == 2 && 2 * L * 4 < 128) {
-                    if (int rc = arena.alloc(&bas_padded, nk * 128)) return rc;
-                    if (int rc = MsmPairLaunch<C>::pad_bases(bas, nk, bas_padded, st)) return rc;
-                }
                 for (int w0 = 0; w0 < g.W; w0 += gw) {
                     const int w1 = std::min(g.W, w0 + gw);
                     const size_t b0 = (size_t)w0 * g.nb, b1 = (w1 == g.W) ? nb_total : (size_t)w1 * g.nb;
-                    if (int rc = reduce_group(bas, bas_padded, b0, b1, upto[w1] - upto[w0], levels, target)) return rc;
+                    if (int rc = reduce_group(bas, b0, b1, upto[w1] - upto[w0], levels, target)) return rc;
                 }
-                arena.release(bas_padded);
             }
         }
         if (chunks_done > 0) {

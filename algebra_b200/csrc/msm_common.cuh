@@ -159,11 +159,9 @@ template <int L> __device__ __forceinline__ void store_xyzz(uint32_t *p, const X
 
 // ---- launchers (definitions: msm_k_pair.cuh / msm_k_acc.cuh / msm_k_red.cuh; instantiations: msm_inst_*.cu) ----
 template <class C> struct MsmPairLaunch {
-    // one batched-affine level over the buckets [0, nbg): variant 1 = thread-contiguous batches, 2 = warp-interleaved + cp.async
-    static int run(int variant, bool first, const uint32_t *bases, const uint32_t *src, const uint32_t *offsets_in, const uint32_t *offsets_out,
-                   const uint32_t *pairmap, uint32_t nbg, uint32_t batch, size_t out_cap, uint32_t *out, int shared_inv, int stagger, uint32_t base_stride, cudaStream_t st);
-    // copy of the bases with one point per 128-byte line (base_stride = 32 words); only for points of <= 128 bytes
-    static int pad_bases(const uint32_t *bases, size_t n, uint32_t *padded, cudaStream_t st);
+    // one batched-affine level over the buckets [0, nbg) (first: the inputs are the bases, gathered through the sorted indices `src`)
+    static int run(bool first, const uint32_t *bases, const uint32_t *src, const uint32_t *offsets_out, const uint32_t *pairmap, uint32_t nbg,
+                   uint32_t batch, size_t out_cap, uint32_t *out, cudaStream_t st);
 };
 template <class C> struct MsmAccLaunch {
     // signed digits of every window, window-major (digits: g.W * nk words)

@@ -1,18 +1,16 @@
-// msm_k_pair.cuh — batched-affine pair-add kernels (both generations) and their launcher.
+// msm_k_pair.cuh — batched-affine pair-add kernel and its launcher.
 #pragma once
-#include <algorithm>
-#include <cstdlib>
 #include "msm_common.cuh"
 
 namespace ab200 {
 
 template <class F, bool FIRST>
 __device__ __forceinline__ void pair_load_point(uint32_t *x, uint32_t *y, const uint32_t *__restrict__ bases, const uint32_t *__restrict__ src,
-                                                uint32_t k, uint32_t base_stride = 2 * F::L) {
+                                                uint32_t k) {
     constexpr int L = F::L;
     if (FIRST) {
         const uint32_t e = __ldg(src + k);
-        const uint32_t *bp = bases + (size_t)(e & 0x7fffffffu) * base_stride;
+        const uint32_t *bp = bases + (size_t)(e & 0x7fffffffu) * (2 * L);
         load_limbs_nc<L>(x, bp);
         load_limbs_nc<L>(y, bp + L);
         F::cneg(y, y, (e >> 31) != 0);   // -(0,0) stays (0,0)
@@ -21,13 +19,6 @@ __device__ __forceinline__ void pair_load_point(uint32_t *x, uint32_t *y, const 
         load_limbs_nc<L>(x, bp);
         load_limbs_nc<L>(y, bp + L);
     }
-}
-// x coordinate only (the forward pass needs y only for the rare degenerate pairs)
-template <class F, bool FIRST>
-__device__ __forceinline__ void pair_load_x(uint32_t *x, const uint32_t *__restrict__ bases, const uint32_t *__restrict__ src, uint32_t k) {
-    constexpr int L = F::L;
-    const uint32_t *bp = FIRST ? bases + (size_t)(__ldg(src + k) & 0x7fffffffu) * (2 * L) : src + (size_t)k * (2 * L);
-    load_limbs_nc<L>(x, bp);
 }
 
 enum { PAIR_PASS1 = 0, PAIR_PASS2 = 1, PAIR_INF = 2, PAIR_ADD = 3, PAIR_DBL = 4 };
@@ -54,12 +45,8 @@ template <class F> __device__ __forceinline__ int pair_classify(uint32_t *den, c
 // peels the 128 inverses back out; every thread then picks up 1/run of its own product.  A per-thread inversion costs ~570
 // multiplications of issue time PER WARP; this costs ~590 per BLOCK, i.e. a quarter — which is what allows short batches.
 // `sm` holds 128 * L words (word i of thread t at sm[i * 128 + t]); all 128 threads of the block must call this.
-// Fp::inv_lowlat (4-bit windows + symmetric squaring) is available for the block inversion but off by default: its table lives in
-// local memory and sqr_sos has more carry-ripple adds than mul(a, a); the plain square-and-multiply stays.
-#ifndef AB_BLOCK_INVERSE_LOWLAT
-#define AB_BLOCK_INVERSE_LOWLAT 0
-#endif
-static constexpr bool kBlockInverseLowLatency = AB_BLOCK_INVERSE_LOWLAT != 0;
+// The inversion is the plain square-and-multiply F::inv, not Fp::inv_lowlat (4-bit windows + symmetric squaring): the latter's
+// table lives in local memory and sqr_sos has more carry-ripple adds than mul(a, a).
 template <class F> __device__ __forceinline__ void shfl_limbs(uint32_t *r, const uint32_t *a, int src_lane) {
 #pragma unroll
     for (int i = 0; i < F::L; i++) r[i] = __shfl_sync(0xffffffffu, a[i], src_lane);
@@ -95,8 +82,7 @@ template <class F> __device__ __noinline__ void block_inverse(uint32_t *inv, con
         }
         uint32_t I[L];
         shfl_limbs<F>(y, P, 31);
-        if (kBlockInverseLowLatency) F::inv_lowlat(I, y);   // 1 / (product of all 128), computed redundantly by the 32 lanes
-        else F::inv(I, y);
+        F::inv(I, y);                                 // 1 / (product of all 128), computed redundantly by the 32 lanes
         shfl_limbs<F>(y, P, lane ? lane - 1 : 0);
         if (lane) F::mul(I, I, y);                    // ... times the products of the other lanes = 1 / a3
         shfl_limbs<F>(y, S, lane < 31 ? lane + 1 : 31);
@@ -111,159 +97,31 @@ template <class F> __device__ __noinline__ void block_inverse(uint32_t *inv, con
     __syncthreads();
 #pragma unroll
     for (int i = 0; i < L; i++) inv[i] = sm[i * 128 + tid];
-    __syncthreads();   // `sm` may be reused by the caller (the staging strips of the second-generation kernel)
+    __syncthreads();   // `sm` may be reused by the caller (the staging strips of the pair-add kernel)
 }
 
-// Latency hiding in this kernel is left to occupancy (128 registers -> 16 warps per SM) rather than to next-slot operands held in
-// registers (198 registers, 8 warps per SM) or a prefetch.global.L2 of them (which fetches whole 128-byte lines for 96-byte points).
-template <class C, bool FIRST, int MINB>
-__global__ void __launch_bounds__(128, MINB) msm_pair_add_kernel(const uint32_t *__restrict__ bases, const uint32_t *__restrict__ src,
-                                                           const uint32_t *__restrict__ offsets_in, const uint32_t *__restrict__ offsets_out,
-                                                           uint32_t total_buckets, uint32_t batch, uint32_t *__restrict__ out,
-                                                           uint32_t num_threads, int shared_inv) {
-    using F = typename C::F;
-    constexpr int L = F::L;
-    __shared__ uint32_t s_inv[128 * L];
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    const uint32_t M = __ldg(offsets_out + total_buckets);
-    const uint64_t lo64 = (uint64_t)t * batch;
-    const bool active = t < num_threads && lo64 < M;
-    if (!active && !shared_inv) return;   // (with the block-shared inversion every thread has to reach the barriers)
-    const uint32_t lo = (uint32_t)min((uint64_t)M, lo64), hi = (uint32_t)min((uint64_t)M, lo64 + batch);
-    uint32_t bl = 0, br = total_buckets;   // last b with offsets_out[b] <= lo
-    while (br - bl > 1) {
-        uint32_t mid = bl + ((br - bl) >> 1);
-        if (__ldg(offsets_out + mid) <= lo) bl = mid; else br = mid;
-    }
-    uint32_t x1[L], y1[L], x2[L], y2[L], den[L], run[L];
-    F::set_one(run);
-    // walk state = the bucket owning the NEXT slot (one ahead of the slot being computed)
-    uint32_t b = bl, out_end = __ldg(offsets_out + b + 1), out_beg = __ldg(offsets_out + b), in_beg = __ldg(offsets_in + b),
-             in_end = __ldg(offsets_in + b + 1);
-    // ---- forward: running product of the denominators, parked in the x-half of each output slot (x coordinates only)
-    uint32_t k = in_beg + 2 * (lo - out_beg);
-    bool has2 = k + 1 < in_end;
-    for (uint32_t p = lo; p < hi; p++) {
-        uint32_t kn = 0;
-        bool has2n = false;
-        if (p + 1 < hi) {
-            while (p + 1 >= out_end) {
-                b++;
-                out_beg = out_end;
-                out_end = __ldg(offsets_out + b + 1);
-                in_beg = __ldg(offsets_in + b);
-                in_end = __ldg(offsets_in + b + 1);
-            }
-            kn = in_beg + 2 * (p + 1 - out_beg);
-            has2n = kn + 1 < in_end;
-        }
-        if (has2) {
-            pair_load_x<F, FIRST>(x1, bases, src, k);
-            pair_load_x<F, FIRST>(x2, bases, src, k + 1);
-            if (limbs_is_zero<L>(x1) || limbs_is_zero<L>(x2) || limbs_eq<L>(x1, x2)) {   // rare: identity operand / equal x
-                pair_load_point<F, FIRST>(x1, y1, bases, src, k);
-                pair_load_point<F, FIRST>(x2, y2, bases, src, k + 1);
-                const int kind = pair_classify<F>(den, x1, y1, x2, y2, true);
-                if (kind >= PAIR_ADD) F::mul(run, run, den);
-            } else {
-                F::sub(den, x2, x1);
-                F::mul(run, run, den);
-            }
-        }
-        store_limbs<L>(out + (size_t)p * (2 * L), run);
-        k = kn;
-        has2 = has2n;
-    }
-    uint32_t inv[L];
-    if (shared_inv) block_inverse<F>(inv, run, s_inv);
-    else F::inv(inv, run);
-    // ---- backward: peel the inverses off and write the sums; the walk state now sits on the bucket of slot hi-1
-    k = in_beg + 2 * (hi - 1 - out_beg);
-    has2 = k + 1 < in_end;
-    for (uint32_t p = hi; p-- > lo;) {
-        uint32_t kn = 0;
-        bool has2n = false;
-        if (p > lo) {
-            while (p - 1 < out_beg) {
-                b--;
-                out_end = out_beg;
-                out_beg = __ldg(offsets_out + b);
-                in_beg = __ldg(offsets_in + b);
-                in_end = __ldg(offsets_in + b + 1);
-            }
-            kn = in_beg + 2 * (p - 1 - out_beg);
-            has2n = kn + 1 < in_end;
-        }
-        pair_load_point<F, FIRST>(x1, y1, bases, src, k);
-        if (has2) pair_load_point<F, FIRST>(x2, y2, bases, src, k + 1);
-        const int kind = pair_classify<F>(den, x1, y1, x2, y2, has2);
-        uint32_t *o = out + (size_t)p * (2 * L);
-        if (kind >= PAIR_ADD) {
-            uint32_t dinv[L], lam[L], t3[L];
-            if (p > lo) { load_limbs<L>(t3, out + (size_t)(p - 1) * (2 * L)); F::mul(dinv, inv, t3); }   // inv * prefix_{p-1} = 1/den
-            else limbs_copy<L>(dinv, inv);
-            F::mul(inv, inv, den);
-            if (kind == PAIR_ADD) {
-                F::sub(lam, y2, y1);
-            } else {                      // doubling: slope = 3 x^2 / (2 y)
-                F::sqr(lam, x1);
-                F::dbl(t3, lam);
-                F::add(lam, lam, t3);
-                limbs_copy<L>(x2, x1);
-            }
-            F::mul(lam, lam, dinv);
-            F::sqr(t3, lam);
-            F::sub(t3, t3, x1);
-            F::sub(t3, t3, x2);           // x3
-            F::sub(x2, x1, t3);
-            F::mul(x2, lam, x2);
-            F::sub(x2, x2, y1);           // y3 = lam (x1 - x3) - y1
-            store_limbs<L>(o, t3);
-            store_limbs<L>(o + L, x2);
-        } else if (kind == PAIR_PASS1) {
-            store_limbs<L>(o, x1);
-            store_limbs<L>(o + L, y1);
-        } else if (kind == PAIR_PASS2) {
-            store_limbs<L>(o, x2);
-            store_limbs<L>(o + L, y2);
-        } else {
-            F::set_zero(x1);
-            store_limbs<L>(o, x1);
-            store_limbs<L>(o + L, x1);
-        }
-        k = kn;
-        has2 = has2n;
-    }
-}
-
-// bucket b = tail[t0] + head[t0+1] + ... + head[t1], t1 = task holding the bucket's last entry.
 // ------------------------------------------------------------------------------------------------
-// Pair-add, second generation: warp-interleaved slots + asynchronous operand staging.
+// Pair-add: warp-interleaved slots + asynchronous operand staging.
 //   * a WARP owns 32*batch consecutive output slots and lane l takes slots l, l+32, l+64, ... — every Montgomery-trick chain is
 //     still private to one thread, but the 32 lanes of a load/store touch 32 consecutive slots (coalesced streaming for the
 //     levels >= 2 and for the parked prefix products);
 //   * the operands of the NEXT slot are fetched with cp.async (LDGSTS) into a per-thread shared-memory strip while the current
-//     slot's multiplications run, so the random 96-byte gathers of level 1 no longer stall the integer pipe and cost no registers;
-//   * slot -> input-pair mapping comes from `pairmap` (msm_pairmap_kernel), not from a per-thread bucket walk.
-// Same arithmetic, same degenerate-pair handling and same output layout as msm_pair_add_kernel.
+//     slot's multiplications run, so the random 96-byte gathers of level 1 do not stall the integer pipe and cost no registers;
+//   * slot -> input-pair mapping comes from `pairmap` (msm_pairmap_kernel);
+//   * the running products of the 128 threads of a block share one field inversion (block_inverse).
 // ------------------------------------------------------------------------------------------------
-// CA = true: cp.async.ca (allocates in L1: the three 16-byte chunks of a 48-byte coordinate, and x then y of a point, hit the line
-// the first chunk brought in); CA = false: cp.async.cg (L2 only)
-template <bool CA> __device__ __forceinline__ void cp_async16(uint32_t saddr, const void *g) {
-    if (CA) asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(saddr), "l"(g) : "memory");
-    else asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(saddr), "l"(g) : "memory");
+// cp.async.ca allocates in L1: the three 16-byte chunks of a 48-byte coordinate, and x then y of a point, hit the line the first
+// chunk brought in
+__device__ __forceinline__ void cp_async16(uint32_t saddr, const void *g) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(saddr), "l"(g) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-#ifndef AB_PAIR_CPASYNC_CA
-#define AB_PAIR_CPASYNC_CA 1
-#endif
-static constexpr bool kPairCpAsyncCA = AB_PAIR_CPASYNC_CA != 0;
 // per-thread strip: element e, 16-byte chunk j of thread t lives at uint4 index (e*(L/4) + j)*128 + t (conflict-free)
-template <int L, bool CA> __device__ __forceinline__ void strip_fetch(uint32_t sbase, int e, const uint32_t *g) {
+template <int L> __device__ __forceinline__ void strip_fetch(uint32_t sbase, int e, const uint32_t *g) {
 #pragma unroll
-    for (int j = 0; j < L / 4; j++) cp_async16<CA>(sbase + ((uint32_t)((e * (L / 4) + j) * 128 + threadIdx.x) << 4), g + 4 * j);
+    for (int j = 0; j < L / 4; j++) cp_async16(sbase + ((uint32_t)((e * (L / 4) + j) * 128 + threadIdx.x) << 4), g + 4 * j);
 }
 template <int L> __device__ __forceinline__ void strip_read(uint32_t *r, const uint4 *sm, int e) {
 #pragma unroll
@@ -273,40 +131,25 @@ template <int L> __device__ __forceinline__ void strip_read(uint32_t *r, const u
     }
 }
 
-// pairmap[p] = (index of the first input entry of output slot p) | (the slot has a second entry) << 31.
-// One block per 1024 consecutive slots: two threads locate the first and last bucket of the block's slot range, the bucket
-// offsets in between are staged in shared memory and every slot finds its bucket by a short binary search there (any bucket
-template <class C, bool FIRST, int MINB>
-__global__ void __launch_bounds__(128, MINB) msm_pair_add2_kernel(const uint32_t *__restrict__ bases, const uint32_t *__restrict__ src,
-                                                                const uint32_t *__restrict__ pairmap, const uint32_t *__restrict__ offsets_out,
-                                                                uint32_t nb, uint32_t batch, uint32_t *__restrict__ out, int shared_inv, int stagger,
-                                                                uint32_t base_stride) {
+template <class C, bool FIRST>
+__global__ void __launch_bounds__(128, C::PAIR_MINB) msm_pair_add_kernel(const uint32_t *__restrict__ bases, const uint32_t *__restrict__ src,
+                                                                        const uint32_t *__restrict__ pairmap, const uint32_t *__restrict__ offsets_out,
+                                                                        uint32_t nb, uint32_t batch, uint32_t *__restrict__ out) {
     using F = typename C::F;
     constexpr int L = F::L;
-    uint64_t stagger_base = 0;
     extern __shared__ uint4 strip[];
     const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(strip);
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t M = __ldg(offsets_out + nb);
-    // Staggered batches: the four blocks of a group (blockIdx & 3) get batches of 100 / 85 / 70 / 55 % of `batch`, so that blocks
-    // resident on one SM drift out of phase — otherwise every block of a wave reaches its (single-warp) block inversion at the same
-    // time and the SM runs on a quarter of its warps for ~10 % of the kernel (ncu: 1.1 warps per issue stalled on the barrier).
-    if (stagger) {
-        const uint32_t r4 = blockIdx.x & 3, b0 = batch, b1 = max(8u, batch * 17 / 20), b2 = max(8u, batch * 14 / 20), b3 = max(8u, batch * 11 / 20);
-        const uint32_t mine = r4 == 0 ? b0 : r4 == 1 ? b1 : r4 == 2 ? b2 : b3;
-        const uint32_t before = r4 == 0 ? 0 : r4 == 1 ? b0 : r4 == 2 ? b0 + b1 : b0 + b1 + b2;
-        stagger_base = ((uint64_t)(blockIdx.x >> 2) * (b0 + b1 + b2 + b3) + before) * 128;
-        batch = mine;
-    }
-    const uint64_t w_lo = (stagger ? stagger_base : (uint64_t)blockIdx.x * 128 * batch) + (uint64_t)(threadIdx.x >> 5) * 32 * batch;
+    const uint64_t w_lo = (uint64_t)blockIdx.x * 128 * batch + (uint64_t)(threadIdx.x >> 5) * 32 * batch;
+    // a lane without slots still runs to block_inverse: every thread of the block has to reach its barriers
     const bool active = w_lo + lane < M;
-    if (!active && !shared_inv) return;   // (with the block-shared inversion every thread has to reach the barriers)
     const uint32_t w_hi = (uint32_t)min((uint64_t)M, w_lo + (uint64_t)32 * batch);
     const uint32_t p0 = active ? (uint32_t)w_lo + lane : 0;
     const uint32_t cnt = active ? (w_hi - p0 + 31) >> 5 : 0;   // slots p0 + 32*i, i < cnt
     // address of the point behind input entry `k` (FIRST: through the sorted index, e = index | sign << 31)
     auto point = [&](uint32_t k, uint32_t e) -> const uint32_t * {
-        return FIRST ? bases + (size_t)(e & 0x7fffffffu) * base_stride : src + (size_t)k * (2 * L);   // base_stride: 2L words, or 32 (padded to a line)
+        return FIRST ? bases + (size_t)(e & 0x7fffffffu) * (2 * L) : src + (size_t)k * (2 * L);
     };
     uint32_t x1[L], y1[L], x2[L], y2[L], den[L], run[L];
     // software pipeline over the slots of this lane: (m, e1, e2) describe a slot (pairmap word and, for FIRST, the two sorted
@@ -319,7 +162,7 @@ __global__ void __launch_bounds__(128, MINB) msm_pair_add2_kernel(const uint32_t
     m_c = __ldg(pairmap + p0);
     if (FIRST) { e1_c = __ldg(src + (m_c & 0x7fffffffu)); if (m_c >> 31) e2_c = __ldg(src + (m_c & 0x7fffffffu) + 1); }
     // (forward uses strip elements {0,2} for even slots and {1,3} for odd ones: a true double buffer)
-    if (m_c >> 31) { strip_fetch<L, kPairCpAsyncCA>(sbase, 0, point(m_c & 0x7fffffffu, e1_c)); strip_fetch<L, kPairCpAsyncCA>(sbase, 2, point((m_c & 0x7fffffffu) + 1, e2_c)); }
+    if (m_c >> 31) { strip_fetch<L>(sbase, 0, point(m_c & 0x7fffffffu, e1_c)); strip_fetch<L>(sbase, 2, point((m_c & 0x7fffffffu) + 1, e2_c)); }
     cp_async_commit();
     if (cnt > 1) {
         m_n = __ldg(pairmap + p0 + 32);
@@ -332,8 +175,8 @@ __global__ void __launch_bounds__(128, MINB) msm_pair_add2_kernel(const uint32_t
         const int eb = (int)(i & 1);
         if (has2) { strip_read<L>(x1, strip, eb); strip_read<L>(x2, strip, 2 + eb); }
         if (i + 1 < cnt && (m_n >> 31)) {
-            strip_fetch<L, kPairCpAsyncCA>(sbase, 1 - eb, point(m_n & 0x7fffffffu, e1_n));
-            strip_fetch<L, kPairCpAsyncCA>(sbase, 3 - eb, point((m_n & 0x7fffffffu) + 1, e2_n));
+            strip_fetch<L>(sbase, 1 - eb, point(m_n & 0x7fffffffu, e1_n));
+            strip_fetch<L>(sbase, 3 - eb, point((m_n & 0x7fffffffu) + 1, e2_n));
         }
         cp_async_commit();
         uint32_t e1_nn = 0, e2_nn = 0, m_n3 = 0;
@@ -342,8 +185,8 @@ __global__ void __launch_bounds__(128, MINB) msm_pair_add2_kernel(const uint32_t
         if (has2) {
             if (limbs_is_zero<L>(x1) || limbs_is_zero<L>(x2) || limbs_eq<L>(x1, x2)) {   // rare: identity operand / equal x
                 const uint32_t k = m_c & 0x7fffffffu;
-                pair_load_point<F, FIRST>(x1, y1, bases, src, k, base_stride);
-                pair_load_point<F, FIRST>(x2, y2, bases, src, k + 1, base_stride);
+                pair_load_point<F, FIRST>(x1, y1, bases, src, k);
+                pair_load_point<F, FIRST>(x2, y2, bases, src, k + 1);
                 const int kind = pair_classify<F>(den, x1, y1, x2, y2, true);
                 if (kind >= PAIR_ADD) F::mul(run, run, den);
             } else {
@@ -358,22 +201,21 @@ __global__ void __launch_bounds__(128, MINB) msm_pair_add2_kernel(const uint32_t
     }
     }
     uint32_t inv[L];
-    if (shared_inv) block_inverse<F>(inv, run, reinterpret_cast<uint32_t *>(strip));   // (no copy is in flight here: the strips are free)
-    else F::inv(inv, run);
+    block_inverse<F>(inv, run, reinterpret_cast<uint32_t *>(strip));   // (no copy is in flight here: the strips are free)
     if (!cnt) return;
 
     // ---------------- backward: peel the inverses off and write the sums; strip elements 0..3 = x1, y1, x2, y2, 4 = prefix
     auto fetch_bwd = [&](uint32_t m, uint32_t e1, uint32_t e2, uint32_t i) {   // operands of slot i and the prefix parked in slot i-1
         const uint32_t k = m & 0x7fffffffu;
         const uint32_t *a = point(k, e1);
-        strip_fetch<L, kPairCpAsyncCA>(sbase, 0, a);
-        strip_fetch<L, kPairCpAsyncCA>(sbase, 1, a + L);
+        strip_fetch<L>(sbase, 0, a);
+        strip_fetch<L>(sbase, 1, a + L);
         if (m >> 31) {
             const uint32_t *b = point(k + 1, e2);
-            strip_fetch<L, kPairCpAsyncCA>(sbase, 2, b);
-            strip_fetch<L, kPairCpAsyncCA>(sbase, 3, b + L);
+            strip_fetch<L>(sbase, 2, b);
+            strip_fetch<L>(sbase, 3, b + L);
         }
-        if (i > 0) strip_fetch<L, kPairCpAsyncCA>(sbase, 4, out + (size_t)(p0 + 32 * (i - 1)) * (2 * L));
+        if (i > 0) strip_fetch<L>(sbase, 4, out + (size_t)(p0 + 32 * (i - 1)) * (2 * L));
     };
     m_c = __ldg(pairmap + p0 + 32 * (cnt - 1));
     e1_c = e2_c = e1_n = e2_n = 0;
@@ -443,58 +285,16 @@ __global__ void __launch_bounds__(128, MINB) msm_pair_add2_kernel(const uint32_t
     }
 }
 
-// bases (2L words each, dense) -> one point per 128-byte line (G1 of BLS12-381: 96 -> 128 bytes): a level-1 gather then touches exactly
-// one line instead of 1.5 on average
-template <int L> __global__ void __launch_bounds__(256) msm_pad_bases_kernel(const uint4 *__restrict__ in, size_t n, uint4 *__restrict__ out) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-#pragma unroll
-    for (int j = 0; j < 2 * L / 4; j++) out[i * 8 + j] = __ldg(in + i * (2 * L / 4) + j);
-}
-template <class C> int MsmPairLaunch<C>::pad_bases(const uint32_t *bases, size_t n, uint32_t *padded, cudaStream_t st) {
-    constexpr int L = C::F::L;
-    if constexpr (2 * L * 4 <= 128) {
-        msm_pad_bases_kernel<L><<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const uint4 *)bases, n, (uint4 *)padded);
-        AB_LAUNCHED();
-        return 0;
-    } else {
-        set_last_error("pad_bases: points larger than one line");
-        return B200_EINVAL;
-    }
-}
-
 template <class C>
-int MsmPairLaunch<C>::run(int variant, bool first, const uint32_t *bases, const uint32_t *src, const uint32_t *offsets_in, const uint32_t *offsets_out,
-                          const uint32_t *pairmap, uint32_t nbg, uint32_t batch, size_t out_cap, uint32_t *out, int shared_inv, int stagger, uint32_t base_stride, cudaStream_t st) {
+int MsmPairLaunch<C>::run(bool first, const uint32_t *bases, const uint32_t *src, const uint32_t *offsets_out, const uint32_t *pairmap, uint32_t nbg,
+                          uint32_t batch, size_t out_cap, uint32_t *out, cudaStream_t st) {
     constexpr int L = C::F::L;
-    if (!base_stride) base_stride = 2 * L;
-    static const int l1_minb = [] { const char *e = getenv("B200_MSM_L1_MINB"); return e ? atoi(e) : 4; }();
-    if (variant == 2) {
-        unsigned pg;
-        if (stagger) {   // groups of four blocks with batches b, 0.85 b, 0.7 b, 0.55 b (see the kernel)
-            const size_t S = (size_t)batch + std::max(8u, batch * 17 / 20) + std::max(8u, batch * 14 / 20) + std::max(8u, batch * 11 / 20);
-            pg = (unsigned)(4 * ((out_cap + 128 * S - 1) / (128 * S)));
-        } else {
-            const size_t warps = (out_cap + (size_t)32 * batch - 1) / ((size_t)32 * batch);
-            pg = (unsigned)((warps + 3) / 4);
-        }
-        const size_t smem = (size_t)5 * (L / 4) * 128 * 16;
-        if (first && l1_minb == 5 && C::PAIR_MINB == 4) {   // experiment: level 1 with 5 resident blocks (<= 102 registers)
-            AB_CUDA(cudaFuncSetAttribute(msm_pair_add2_kernel<C, true, C::PAIR_MINB + 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            msm_pair_add2_kernel<C, true, C::PAIR_MINB + 1><<<pg, 128, smem, st>>>(bases, src, pairmap, offsets_out, nbg, batch, out, shared_inv, stagger, base_stride);
-        } else if (first) {
-            AB_CUDA(cudaFuncSetAttribute(msm_pair_add2_kernel<C, true, C::PAIR_MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            msm_pair_add2_kernel<C, true, C::PAIR_MINB><<<pg, 128, smem, st>>>(bases, src, pairmap, offsets_out, nbg, batch, out, shared_inv, stagger, base_stride);
-        } else {
-            AB_CUDA(cudaFuncSetAttribute(msm_pair_add2_kernel<C, false, C::PAIR_MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            msm_pair_add2_kernel<C, false, C::PAIR_MINB><<<pg, 128, smem, st>>>(bases, src, pairmap, offsets_out, nbg, batch, out, shared_inv, stagger, base_stride);
-        }
-    } else {
-        const uint32_t nthreads = (uint32_t)((out_cap + batch - 1) / batch);
-        const unsigned pg = (nthreads + 127) / 128;
-        if (first) msm_pair_add_kernel<C, true, C::PAIR_MINB><<<pg, 128, 0, st>>>(bases, src, offsets_in, offsets_out, nbg, batch, out, nthreads, shared_inv);
-        else msm_pair_add_kernel<C, false, C::PAIR_MINB><<<pg, 128, 0, st>>>(bases, src, offsets_in, offsets_out, nbg, batch, out, nthreads, shared_inv);
-    }
+    const size_t warps = (out_cap + (size_t)32 * batch - 1) / ((size_t)32 * batch);
+    const unsigned pg = (unsigned)((warps + 3) / 4);
+    const size_t smem = (size_t)5 * (L / 4) * 128 * 16;
+    auto kernel = first ? msm_pair_add_kernel<C, true> : msm_pair_add_kernel<C, false>;
+    AB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<pg, 128, smem, st>>>(bases, src, pairmap, offsets_out, nbg, batch, out);
     AB_LAUNCHED();
     return 0;
 }

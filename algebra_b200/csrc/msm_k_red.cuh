@@ -87,33 +87,12 @@ __global__ void __launch_bounds__(128) msm_sum_partials_kernel(const uint32_t *_
     }
 }
 
-// total = sum_w 2^(c*w) * S_w by Horner (:489-502); Jacobian result (x, y, z) -> out (3L words)
-template <class C> __global__ void msm_window_combine_kernel(const uint32_t *__restrict__ window_sums, int W, int c, uint32_t *__restrict__ out) {
-    using F = typename C::F;
-    using E = Ec<F>;
-    constexpr int L = F::L;
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    typename E::J total;
-    E::jac_set_zero(total);
-    for (int w = W - 1; w >= 0; w--) {
-        typename E::B b;
-        typename E::J j;
-        load_xyzz<L>(b, window_sums + (size_t)w * (4 * L));
-        E::xyzz_to_jac(j, b);
-        E::jac_add(total, j);  // Projective += &Bucket (bucket.rs:345-359)
-        if (w > 0)
-            for (int d = 0; d < c; d++) E::jac_dbl(total);
-    }
-    store_limbs<L>(out, total.x);
-    store_limbs<L>(out + L, total.y);
-    store_limbs<L>(out + 2 * L, total.z);
-}
-
-// The same Horner combine with the independent field multiplications of every point operation spread over the lanes of one
+// Window combine: total = sum_w 2^(c*w) * S_w by Horner (:489-502), Projective += &Bucket (bucket.rs:345-359); Jacobian result
+// (x, y, z) -> out (3L words).  The independent field multiplications of every point operation are spread over the lanes of one
 // warp (operands in shared-memory slots): a Jacobian doubling is 3 dependent rounds of multiplications instead of 7, an
 // addition 6 instead of 16.  c*(W-1) doublings in sequence are the latency floor of this step, a
 // large share of a small MSM; the exceptional cases (equal / opposite operands)
-// fall back to the one-thread formulas.  Same group element as msm_window_combine_kernel.
+// fall back to the one-thread formulas (Ec::jac_add).
 template <class F> struct CoopSlots {
     static constexpr int L = F::L;
     uint32_t *sm;

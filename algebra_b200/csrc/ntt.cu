@@ -19,10 +19,6 @@
 // + (m-1) segment-twiddle multiplies.  2^24 = 256^3: 3*3.5 + 2 = 12.5 modmuls/element (136 IMAD.WIDE each).
 // HBM traffic: m reads + m writes of the data + (m-1) table reads (L2-resident except the pass-1 table).
 // 1/n of the inverse transform is folded into the pass-1 table; coset scaling is a separate element-wise kernel.
-#include <cuda.h>
-#include <algorithm>
-#include <cstdlib>
-#include <cstring>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -47,7 +43,7 @@ struct NttPassParams {
 };
 
 // shared-memory tile: two 16-byte planes so that consecutive elements are consecutive uint4 (conflict-free)
-template <class P, bool FUSE_LAST2>
+template <class P>
 __global__ void __launch_bounds__(512, 2) ntt_pass_kernel(const uint4 *in, uint4 *out, NttPassParams pp) {
     using F = Fp<P>;
     extern __shared__ uint4 smem[];
@@ -102,7 +98,7 @@ __global__ void __launch_bounds__(512, 2) ntt_pass_kernel(const uint4 *in, uint4
     {
         const bool active = tid < tile / 2;
         const int g = tid & (G - 1), u = tid >> logG;
-        const int radix2_stages = (FUSE_LAST2 && r >= 2) ? r - 2 : r;
+        const int radix2_stages = r >= 2 ? r - 2 : r;
         for (int s = 0; s < radix2_stages; s++) {
             if (active) {
                 const int gaplog = r - 1 - s;
@@ -129,7 +125,7 @@ __global__ void __launch_bounds__(512, 2) ntt_pass_kernel(const uint4 *in, uint4
             }
             __syncthreads();
         }
-        if (FUSE_LAST2 && r >= 2) {
+        if (r >= 2) {
             if (tid < tile / 4) {   // group (q, g): rows 4q .. 4q+3 of column g
                 const int q = tid >> logG, base = ((4 * q) << logG) + g;
                 uint32_t x[4][8], t[8], w[8];
@@ -201,219 +197,6 @@ __global__ void __launch_bounds__(512, 2) ntt_pass_kernel(const uint4 *in, uint4
             }
             out[2 * pos] = v0;
             out[2 * pos + 1] = v1;
-        }
-    }
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// Second-generation pass kernel: warp-private tiles staged by the TMA, radix-4 register butterflies.
-//   * A warp owns a tile of 256 elements = C = 256/A adjacent columns of one A-point sub-transform (8 KiB of shared memory),
-//     so the butterfly stages need __syncwarp only — no block barrier anywhere in the kernel.
-//   * Tiles arrive through the Tensor Memory Accelerator: one cp.async.bulk.tensor.3d per tile (box = C columns x A rows of
-//     32-byte elements out of the [segment][row][column] view of the vector; the strided gather is done by the copy engine),
-//     or one contiguous cp.async.bulk for the last pass; completion is signalled on an mbarrier.  Each warp double-buffers:
-//     the tile after next is requested as soon as the last butterfly step has pulled the current tile into registers.
-//   * Stages are fused in pairs (radix 4, 4 elements per lane in registers): half the shared-memory round trips, and the
-//     final pair only needs ONE twiddle multiplication per 4 elements (w = 1 for three of its four butterflies).
-//   * Results go from registers straight to their final position (segment twiddle multiply fused, as before).
-// Persistent grid: 3 blocks of 4 warps per SM, tile t of a pass handled by warp (t mod #warps).
-// ------------------------------------------------------------------------------------------------
-struct Ntt2Params {
-    int log_n, r, logC, log_seg, is_last, m;
-    int radix_log[kMaxPasses];
-    const uint4 *tw_small, *tw_seg;
-    int has_scale;
-    uint32_t scale[8];
-    uint32_t tiles;   // n / 256
-};
-
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    const uint32_t a = (uint32_t)__cvta_generic_to_shared(bar);
-    asm volatile(
-        "{\n.reg .pred p;\nWAIT_%=:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra DONE_%=;\nbra WAIT_%=;\nDONE_%=:\n}" ::"r"(a), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map, int c0, int c1, int c2, uint64_t *bar) {
-    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-                 ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(map), "r"(c0), "r"(c1), "r"(c2),
-                   "r"((uint32_t)__cvta_generic_to_shared(bar)) : "memory");
-}
-__device__ __forceinline__ void bulk_load_1d(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src), "r"(bytes), "r"((uint32_t)__cvta_generic_to_shared(bar)) : "memory");
-}
-
-__device__ __forceinline__ void ld_elem(uint32_t *x, const uint4 *p) {
-    const uint4 a = p[0], b = p[1];
-    x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w; x[4] = b.x; x[5] = b.y; x[6] = b.z; x[7] = b.w;
-}
-__device__ __forceinline__ void ldg_elem(uint32_t *x, const uint4 *p) {
-    const uint4 a = __ldg(p), b = __ldg(p + 1);
-    x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w; x[4] = b.x; x[5] = b.y; x[6] = b.z; x[7] = b.w;
-}
-__device__ __forceinline__ void st_elem(uint4 *p, const uint32_t *x) {
-    p[0] = make_uint4(x[0], x[1], x[2], x[3]);
-    p[1] = make_uint4(x[4], x[5], x[6], x[7]);
-}
-
-// two fused DIF stages on x[0..3] = elements at rows a, a+h, a+2h, a+3h (a = a_hi*4h + a_lo); twiddle table t -> w_256^t
-template <class P, bool LAST> __device__ __forceinline__ void radix4_dif(uint32_t (*x)[8], const uint4 *tw, int a_lo, int h) {
-    using F = Fp<P>;
-    uint32_t t[8], w[8];
-    const int q = 64 / h;   // h <= 64
-    // gap 2h: (x0, x2) with w_{4h}^{a_lo}, (x1, x3) with w_{4h}^{a_lo + h}
-    F::sub(t, x[0], x[2]); F::add(x[0], x[0], x[2]);
-    if (LAST) limbs_copy<8>(x[2], t);
-    else { ldg_elem(w, tw + 2 * (a_lo * q)); F::mul(x[2], t, w); }
-    F::sub(t, x[1], x[3]); F::add(x[1], x[1], x[3]);
-    ldg_elem(w, tw + 2 * ((a_lo + h) * q));
-    F::mul(x[3], t, w);
-    // gap h: (x0, x1) and (x2, x3), both with w_{2h}^{a_lo}
-    if (!LAST) ldg_elem(w, tw + 2 * (a_lo * 2 * q));
-    F::sub(t, x[0], x[1]); F::add(x[0], x[0], x[1]);
-    if (LAST) limbs_copy<8>(x[1], t); else F::mul(x[1], t, w);
-    F::sub(t, x[2], x[3]); F::add(x[2], x[2], x[3]);
-    if (LAST) limbs_copy<8>(x[3], t); else F::mul(x[3], t, w);
-}
-
-// kNtt2Buffers tile buffers of 8 KiB per warp.  1 buffer / 6 blocks of 4 warps per SM (<= 85 registers, final radix-4 groups one after
-// the other, the next tile requested when the second group has been read; 6 x 32 KiB fits the H100's 227 KiB of shared memory) rather
-// than 2 buffers / 3 blocks (both final groups in registers): 12 warps per SM leave the integer pipe idle too often.
-static constexpr int kNtt2Buffers = 1, kNtt2BlocksPerSm = 6;
-static constexpr size_t kNtt2SmemBytes = (size_t)4 * kNtt2Buffers * 8192 + 64;
-
-template <class P>
-__global__ void __launch_bounds__(128, kNtt2BlocksPerSm) ntt2_pass_kernel(const __grid_constant__ CUtensorMap tmap, const uint4 *__restrict__ in,
-                                                                          uint4 *__restrict__ out, Ntt2Params pp) {
-    using F = Fp<P>;
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint4 *buf0 = reinterpret_cast<uint4 *>(smem_raw + (size_t)warp * kNtt2Buffers * 8192);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + (size_t)4 * kNtt2Buffers * 8192) + warp * 2;
-    const int r = pp.r, A = 1 << r, logC = pp.logC, C = 1 << logC;
-    const int logB = pp.log_seg - r, logA1 = pp.radix_log[0];
-    const uint32_t nwarps = gridDim.x * 4, wid = blockIdx.x * 4 + warp;
-    if (lane == 0) {
-        mbar_init(&bars[0], 1);
-        mbar_init(&bars[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    auto request = [&](uint32_t tile, int stage) {   // lane 0 only
-        uint4 *dst = buf0 + stage * 512;
-        mbar_expect_tx(&bars[stage], 8192);
-        if (!pp.is_last) {
-            const int log_cg = logB - logC;                       // column groups per segment
-            const uint32_t cg = tile & ((1u << log_cg) - 1), sigma = tile >> log_cg;
-            tma_load_3d(dst, &tmap, (int)(cg << (logC + 2)), 0, (int)sigma, &bars[stage]);
-        } else {
-            // tile = qg * A1 + g: C consecutive sub-transforms (q = qg*C + rho) of input row block g -> 256 contiguous elements
-            const uint32_t g = tile & ((1u << logA1) - 1), qg = tile >> logA1;
-            const size_t pos = ((size_t)g << (pp.log_n - logA1)) + ((size_t)qg << 8);
-            bulk_load_1d(dst, in + 2 * pos, 8192, &bars[stage]);
-        }
-    };
-    if (lane == 0)
-        for (int b = 0; b < kNtt2Buffers; b++)
-            if (wid + (size_t)b * nwarps < pp.tiles) request(wid + b * nwarps, b);
-    uint32_t it = 0;
-    for (uint32_t tile = wid; tile < pp.tiles; tile += nwarps, it++) {
-        const int stage = it % kNtt2Buffers;
-        uint4 *buf = buf0 + stage * 512;
-        mbar_wait(&bars[stage], (it / kNtt2Buffers) & 1);
-        // element (row a, column c) of the tile: non-last layout [a][c] (TMA box), last layout [c][a] (contiguous runs)
-        auto slot = [&](int a, int c) { return pp.is_last ? ((c << r) + a) : ((a << logC) + c); };
-        int stages_left = r;
-        if (r & 1) {   // one radix-2 stage at gap A/2 (128 butterflies per tile, 4 per lane)
-            const int gap = A >> 1;
-#pragma unroll 1
-            for (int k = 0; k < 4; k++) {
-                const int beta = lane + 32 * k;
-                const int c = pp.is_last ? (beta >> (r - 1)) : (beta & (C - 1));
-                const int j = pp.is_last ? (beta & (gap - 1)) : (beta >> logC);
-                uint32_t x[8], y[8], d[8], w[8];
-                uint4 *plo = buf + 2 * slot(j, c), *phi = buf + 2 * slot(j + gap, c);
-                ld_elem(x, plo); ld_elem(y, phi);
-                F::sub(d, x, y); F::add(x, x, y);
-                ldg_elem(w, pp.tw_small + 2 * (j << (kMaxLogRadix - r)));
-                F::mul(d, d, w);
-                st_elem(plo, x); st_elem(phi, d);
-            }
-            __syncwarp();
-            stages_left--;
-        }
-        // radix-4 steps in shared memory while more than two stages remain
-        int h = 1 << (stages_left - 2);
-        for (; h > 1; h >>= 2) {
-            const int logh = 31 - __clz(h);
-#pragma unroll 1
-            for (int k = 0; k < 2; k++) {
-                const int gam = lane + 32 * k;   // 64 groups: (c, a_hi, a_lo)
-                int c, rest;
-                if (pp.is_last) { c = gam >> (r - 2); rest = gam & ((A >> 2) - 1); }
-                else { c = gam & (C - 1); rest = gam >> logC; }
-                const int a_lo = rest & (h - 1), a0 = ((rest >> logh) << (logh + 2)) + a_lo;
-                uint32_t x[4][8];
-#pragma unroll
-                for (int e = 0; e < 4; e++) ld_elem(x[e], buf + 2 * slot(a0 + e * h, c));
-                radix4_dif<P, false>(x, pp.tw_small, a_lo, h);
-#pragma unroll
-                for (int e = 0; e < 4; e++) st_elem(buf + 2 * slot(a0 + e * h, c), x[e]);
-            }
-            __syncwarp();
-        }
-        // last two stages (h = 1) in registers, one group of four rows at a time; results go straight to global memory, so once the
-        // second group has been read the buffer is free and the next tile is requested
-#pragma unroll 1
-        for (int k = 0; k < 2; k++) {
-            const int gam = lane + 32 * k;
-            int zc, rest;
-            if (pp.is_last) { zc = gam >> (r - 2); rest = gam & ((A >> 2) - 1); }
-            else { zc = gam & (C - 1); rest = gam >> logC; }
-            const int za = rest << 2;
-            uint32_t z[4][8];
-#pragma unroll
-            for (int e = 0; e < 4; e++) ld_elem(z[e], buf + 2 * slot(za + e, zc));
-            if (k == 1) {
-                __syncwarp();
-                if (lane == 0 && tile + (size_t)kNtt2Buffers * nwarps < pp.tiles) request(tile + kNtt2Buffers * nwarps, stage);
-            }
-            radix4_dif<P, true>(z, pp.tw_small, 0, 1);
-#pragma unroll
-            for (int e = 0; e < 4; e++) {
-                const size_t iA = __brev((unsigned)(za + e)) >> (32 - r);   // row a holds sub-transform output bitrev_r(a)
-                size_t pos;
-                if (!pp.is_last) {
-                    const int log_cg = logB - logC;
-                    const size_t cg = tile & ((1u << log_cg) - 1), sigma = tile >> log_cg;
-                    const size_t off = (iA << logB) + (cg << logC) + zc;
-                    pos = (sigma << pp.log_seg) + off;
-                    uint32_t w[8];
-                    ldg_elem(w, pp.tw_seg + 2 * off);
-                    F::mul(z[e], z[e], w);
-                } else {
-                    const size_t g = tile & ((1u << logA1) - 1), q = ((size_t)(tile >> logA1) << logC) + zc;
-                    // position digits (i1 | i2 .. i_{m-1} | i_m)  ->  index i1 + A1*(i2 + A2*(... + A_{m-1}*i_m))
-                    size_t rev = 0, rem = q;
-                    int shift = 0, pv = pp.log_n - logA1 - r;
-                    for (int d = 1; d < pp.m - 1; d++) {
-                        pv -= pp.radix_log[d];
-                        rev += (rem >> pv) << shift;
-                        rem &= ((size_t)1 << pv) - 1;
-                        shift += pp.radix_log[d];
-                    }
-                    pos = g + ((rev + (iA << shift)) << logA1);
-                }
-                st_elem(out + 2 * pos, z[e]);
-            }
         }
     }
 }
@@ -577,68 +360,6 @@ int ntt_clear_cache() {
     return 0;
 }
 
-// cuTensorMapEncodeTiled through the runtime's driver entry point (no link-time dependency on libcuda)
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                                  const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn tensor_map_encoder() {
-    static EncodeTiledFn fn = [] {
-        void *p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) p = nullptr;
-        return (EncodeTiledFn)p;
-    }();
-    return fn;
-}
-struct NttKnobs {
-    int logG = 1, generation = 1, fuse_last2 = 1;
-    NttKnobs() {
-        if (const char *e = getenv("B200_NTT_LOGG")) logG = std::min(3, std::max(0, atoi(e)));   // first-generation kernel: columns per block
-        // generation 1 (block tiles, LDG/STS) is the default, generation 2 (TMA-staged warp tiles) the alternative: the kernel is bound
-        // by the integer pipe, not by tile movement
-        if (const char *e = getenv("B200_NTT_GENERATION")) generation = atoi(e) == 2 ? 2 : 1;
-        if (const char *e = getenv("B200_NTT_FUSE_LAST2")) fuse_last2 = atoi(e) != 0;
-    }
-};
-static const NttKnobs &ntt_knobs() {
-    static const NttKnobs k;
-    return k;
-}
-
-// one pass of the second-generation kernel; `src` viewed as [n/seg][A][B] 32-byte elements = [n/seg][A][4B] u64 for the TMA
-template <class P> static int ntt2_launch_pass(const NttPlan &plan, int t, int log_seg, const uint4 *src, uint4 *dst, bool inverse, cudaStream_t st) {
-    const int log_n = plan.log_n, r = plan.radix_log[t], logB = log_seg - r;
-    Ntt2Params pp;
-    pp.log_n = log_n; pp.r = r; pp.logC = 8 - r; pp.log_seg = log_seg; pp.is_last = (t == plan.m - 1); pp.m = plan.m;
-    for (int i = 0; i < kMaxPasses; i++) pp.radix_log[i] = plan.radix_log[i];
-    pp.tw_small = plan.tw_small; pp.tw_seg = plan.tw_seg[t];
-    pp.has_scale = 0;
-    for (int i = 0; i < 8; i++) pp.scale[i] = plan.scale[i];
-    pp.tiles = (uint32_t)(((size_t)1 << log_n) >> 8);
-    CUtensorMap map;
-    memset(&map, 0, sizeof map);
-    if (!pp.is_last) {
-        EncodeTiledFn enc = tensor_map_encoder();
-        if (!enc) { set_last_error("cuTensorMapEncodeTiled is not available from this driver"); return B200_EINVAL; }
-        const cuuint64_t dims[3] = {(cuuint64_t)4 << logB, (cuuint64_t)1 << r, (cuuint64_t)1 << (log_n - log_seg)};
-        const cuuint64_t strides[2] = {(cuuint64_t)32 << logB, (cuuint64_t)32 << log_seg};   // bytes, dims 1 and 2
-        const cuuint32_t box[3] = {(cuuint32_t)4 << pp.logC, (cuuint32_t)1 << r, 1};
-        const cuuint32_t estr[3] = {1, 1, 1};
-        CUresult cr = enc(&map, CU_TENSOR_MAP_DATA_TYPE_UINT64, 3, (void *)src, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (cr != CUDA_SUCCESS) { set_last_error("cuTensorMapEncodeTiled failed (" + std::to_string((int)cr) + ")"); return B200_EINVAL; }
-    }
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const size_t smem = kNtt2SmemBytes;
-    AB_CUDA(cudaFuncSetAttribute(ntt2_pass_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const unsigned blocks = (unsigned)std::min<size_t>((size_t)sms * kNtt2BlocksPerSm, (pp.tiles + 3) / 4);
-    ntt2_pass_kernel<P><<<blocks, 128, smem, st>>>(map, src, dst, pp);
-    AB_LAUNCHED();
-    (void)inverse;
-    return 0;
-}
-
 template <class P> static int ntt_run(int field, uint4 *d_data, int log_n, bool inverse, const uint64_t *coset, cudaStream_t st) {
     using F = Fp<P>;
     if (log_n > P::TWO_ADICITY) {
@@ -703,15 +424,7 @@ template <class P> static int ntt_run(int field, uint4 *d_data, int log_n, bool 
     uint4 *scratch = nullptr;
     if (plan.m > 1) AB_CUDA(cudaMallocAsync(&scratch, n * 32, st));
     int log_seg = log_n;
-    const bool gen2 = ntt_knobs().generation == 2 && log_n >= 16;   // every pass then has >= 256-element tiles (see ntt2_pass_kernel)
     for (int t = 0; t < plan.m; t++) {
-        if (gen2) {
-            const uint4 *src2 = (t == 0) ? d_data : scratch;
-            uint4 *dst2 = (t == plan.m - 1) ? d_data : scratch;
-            if (int rc = ntt2_launch_pass<P>(plan, t, log_seg, src2, dst2, inverse, st)) return rc;
-            log_seg -= plan.radix_log[t];
-            continue;
-        }
         NttPassParams pp;
         pp.log_n = log_n;
         pp.r = plan.radix_log[t];
@@ -726,7 +439,7 @@ template <class P> static int ntt_run(int field, uint4 *d_data, int log_n, bool 
         const int logB = log_seg - pp.r;
         // G adjacent columns per block.  Small blocks (128-256 threads, 8-16 KB smem) keep ~10 blocks per SM so load/store phases
         // of one block hide behind the butterflies of the others; G=2 keeps 64-byte contiguous runs.
-        int logG = ntt_knobs().logG;
+        int logG = 1;
         if (!pp.is_last) { if (logG > logB) logG = logB; }
         else if (plan.m > 1) { if (logG > plan.radix_log[0]) logG = plan.radix_log[0]; }
         else logG = 0;
@@ -737,8 +450,7 @@ template <class P> static int ntt_run(int field, uint4 *d_data, int log_n, bool 
         const unsigned blocks = (unsigned)(n >> (pp.r + logG));
         const uint4 *src = (t == 0) ? d_data : scratch;
         uint4 *dst = pp.is_last ? d_data : scratch;
-        if (ntt_knobs().fuse_last2) ntt_pass_kernel<P, true><<<blocks, threads, (size_t)tile * 32, st>>>(src, dst, pp);
-        else ntt_pass_kernel<P, false><<<blocks, threads, (size_t)tile * 32, st>>>(src, dst, pp);
+        ntt_pass_kernel<P><<<blocks, threads, (size_t)tile * 32, st>>>(src, dst, pp);
         AB_LAUNCHED();
         log_seg = logB;
     }

@@ -26,7 +26,6 @@ for inverse in (False, True):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(); f(x); e1.record(); torch.cuda.synchronize()
         ts.append(e0.elapsed_time(e1))
-    print(json.dumps({"log_n": a.log_n, "inverse": inverse, "generation": os.environ.get("B200_NTT_GENERATION", "1 (default)"), "best_ms": min(ts),
-                      "mean_ms": sum(ts) / len(ts)}), flush=True)
+    print(json.dumps({"log_n": a.log_n, "inverse": inverse, "best_ms": min(ts), "mean_ms": sum(ts) / len(ts)}), flush=True)
 # (3 + reps) forward then as many inverse transforms restore the input
 print(json.dumps({"roundtrip_ok": bool(torch.equal(x, x0))}))

@@ -26,8 +26,8 @@ for cid, N in ((0, 6), (1, 4), (2, 12)):
         a = ab.into_affine(cid, ab.msm(cid, d_bases, d_s))
         ref = a if ref is None else ref
         assert (a == ref).all()
-    # batched-affine levels forced on at this small size: pairmap + generation-2 pair-add (cp.async strips, block-shared inversion
-    # through shared memory and barriers) and, with B200_MSM_PAIR_VARIANT=1, the generation-1 kernel
+    # batched-affine levels forced on at this small size: pairmap + pair-add (cp.async strips, block-shared inversion through
+    # shared memory and barriers)
     for levels, c in ((1, 5), (2, 6), (3, 4)):
         VB.set_affine_levels(levels)
         VB.set_window(c)
@@ -60,7 +60,7 @@ for cid, N in ((0, 6), (1, 4), (2, 12)):
     co.ifft_in_place(x)
     assert torch.equal(x, x0)
     ab.poly_mul(cid, x[:300], x[300:500])
-    dom16 = ab.Radix2EvaluationDomain.new(cid, 1 << 16)            # >= 2^16: the TMA kernel when B200_NTT_GENERATION=2
+    dom16 = ab.Radix2EvaluationDomain.new(cid, 1 << 16)            # two passes of 256 and 256
     y = torch.empty((1 << 16, 4), dtype=torch.int64, device="cuda")
     _lib.check(L.b200_gen_scalars_dev(cid, 10, 1 << 16, y.data_ptr(), st))
     y0 = y.clone()
