@@ -169,6 +169,8 @@ __global__ void __launch_bounds__(256) msm_pairmap_kernel(const uint32_t *__rest
 // ------------------------------------------------------------------------------------------------
 // Options of a call.  Defaults come from the per-thread setters (b200_set_msm_window / _affine_levels) and, for the tuning
 // knobs without a public setter, from environment variables read ONCE per process (never on the call path).
+// The first MSM of the process builds EnvKnobs; changing a B200_MSM_* variable afterwards has no effect, so a test of a knob
+// must set it in a fresh process before that process's first MSM (tests/test_gpu_msm_paths.py runs one child per setting).
 struct EnvKnobs {
     double level_budget_bytes = 48e9;     // scratch allowed for the affine level arrays (window groups are sized to fit); also capped
                                           // by 60 % of the free device memory at the start of the call, which on an 80 GB H100 is the

@@ -370,19 +370,6 @@ def test_batched_affine_levels(levels):
         M.set_affine_levels(-1)
 
 
-def test_chunked_device_path(monkeypatch):
-    """Device-resident inputs beyond 2^27 pairs are processed as several chunks merged bucket-wise; the hook
-    B200_MSM_FORCE_CHUNKS exercises that path at a testable size."""
-    cid, n = 0, 5000
-    d_bases, d_b, d_s = synth(cid, n, 321)
-    want = expected_from_b(cid, from_dev(d_b), from_dev(d_s))
-    for k in ("3", "7"):
-        monkeypatch.setenv("B200_MSM_FORCE_CHUNKS", k)
-        assert (ab.into_affine(cid, ab.msm(cid, d_bases, d_s)) == want).all()
-    monkeypatch.delenv("B200_MSM_FORCE_CHUNKS")
-    assert (ab.into_affine(cid, ab.msm(cid, d_bases, d_s)) == want).all()
-
-
 @pytest.mark.parametrize("cid,n,c,slices", [(0, 1 << 12, 0, 2), (0, 1 << 12, 9, 3), (0, 3001, 12, 8), (1, 1 << 12, 10, 4), (0, 1 << 12, 2, 5),
                                             (0, 1 << 12, 1, 2), (0, 1 << 16, 0, 8), (0, 1 << 12, 13, 64)])
 def test_bucket_slices_add_up(cid, n, c, slices):

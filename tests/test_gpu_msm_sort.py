@@ -4,8 +4,8 @@ buckets planned from per-group counts, then every bin sorted by bucket in shared
 The bin planner (msm_common.cuh: sort_window / sort_bin_height / sort_bin_of) is compiled for the host and walked as the plan
 kernel walks it: bins tile every window's buckets contiguously and in order, respect the shared-memory capacity and span, and
 fit the grid of the bin-sort kernel.  The GPU tests drive the loads the planner has to cope with — one bucket above the
-capacity, two adjacent heavy buckets in one bin, dense top windows, bucket slices, small scalar kinds, chunked sessions and
-the other curves — and check each result by MSM(b_i*G, s_i) = (sum s_i*b_i mod r)*G."""
+capacity, two adjacent heavy buckets in one bin, dense top windows, bucket slices, small scalar kinds and the other curves
+(chunked sessions: test_gpu_msm_paths.py) — and check each result by MSM(b_i*G, s_i) = (sum s_i*b_i mod r)*G."""
 import ctypes
 import os
 import random
@@ -242,18 +242,6 @@ def test_small_kinds_and_odd_sizes(n):
         limbs[:, 0] = sc
         assert (ab.into_affine(0, fn(0, bh, sc)) == want_linear(0, b, limbs)).all(), bits
     assert (msm_affine(0, d_bases, d_s) == want_linear(0, b, canonical(0, gu.from_dev(d_s)))).all()
-
-
-@pytest.mark.gpu
-def test_forced_chunks(monkeypatch):
-    ab, _lib, M, C, O, gu = _gpu_imports()
-    n = (1 << 16) + 7
-    d_bases, b, d_s = synth(0, n, 505)
-    want = want_linear(0, b, canonical(0, gu.from_dev(d_s)))
-    for k in ("2", "5"):
-        monkeypatch.setenv("B200_MSM_FORCE_CHUNKS", k)
-        assert (msm_affine(0, d_bases, d_s) == want).all(), k
-    monkeypatch.delenv("B200_MSM_FORCE_CHUNKS")
 
 
 @pytest.mark.gpu
