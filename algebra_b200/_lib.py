@@ -44,6 +44,8 @@ SIGNATURES = {
     "b200_ntt_fr": (_c.c_int, [_c.c_int, _vp, _c.c_uint32, _c.c_int, _vp]),
     "b200_ntt_fr_padded": (_c.c_int, [_c.c_int, _vp, _c.c_size_t, _vp, _c.c_uint32, _c.c_int, _vp]),
     "b200_ntt_fr_dev": (_c.c_int, [_c.c_int, _vp, _c.c_uint32, _c.c_int, _vp, _vp]),
+    "b200_ntt_g1": (_c.c_int, [_c.c_int, _vp, _c.c_uint32, _c.c_int, _vp]),
+    "b200_ntt_g1_dev": (_c.c_int, [_c.c_int, _vp, _c.c_uint32, _c.c_int, _vp, _vp]),
     "b200_clear_cache": (_c.c_int, []),
     "b200_poly_mul_size": (_c.c_size_t, [_c.c_int, _c.c_size_t, _c.c_size_t]),
     "b200_poly_mul_fr": (_c.c_int, [_c.c_int, _vp, _c.c_size_t, _vp, _c.c_size_t, _vp]),

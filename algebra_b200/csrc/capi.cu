@@ -11,6 +11,9 @@
 namespace ab200 {
 int ntt_dispatch(int field, void *d_data, uint32_t log_n, int inverse, const uint64_t *coset, cudaStream_t st);
 int ntt_clear_cache();
+int point_ntt_check(int curve, const void *points, uint32_t log_n);
+int point_ntt_coord_words(int curve);
+int point_ntt_dispatch(int curve, void *d_points, uint32_t log_n, int inverse, const uint64_t *coset, cudaStream_t st);
 struct MsmSessionBase {
     virtual ~MsmSessionBase() {}
     virtual int begin(size_t n_total, size_t max_chunk, int kind, cudaStream_t st) = 0;
@@ -530,6 +533,42 @@ int b200_ntt_fr_padded(int field, const uint64_t *in, size_t len_in, uint64_t *o
 }
 int b200_ntt_fr(int field, uint64_t *data, uint32_t log_n, int inverse, const uint64_t *coset_offset) {
     return b200_ntt_fr_padded(field, data, log_n <= 40 ? (size_t)1 << log_n : 0, data, log_n, inverse, coset_offset);
+}
+int b200_ntt_g1_dev(int curve, void *d_points, uint32_t log_n, int inverse, const uint64_t *coset_offset, void *stream) {
+    { int irc = ensure_device_init(); if (irc) return irc; }
+    int rc = point_ntt_dispatch(curve, d_points, log_n, inverse, coset_offset, (cudaStream_t)stream);
+    if (rc) return rc;
+    AB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+    return 0;
+}
+// host-buffer point transform: staged H2D (pinned or pageable), transform in place on the device, D2H
+int b200_ntt_g1(int curve, uint64_t *points, uint32_t log_n, int inverse, const uint64_t *coset_offset) {
+    { int irc = ensure_device_init(); if (irc) return irc; }
+    if (int rc = point_ntt_check(curve, points, log_n)) return rc;
+    const size_t bytes = ((size_t)1 << log_n) * 3 * (size_t)point_ntt_coord_words(curve) * 4;
+    int dev = 0;
+    AB_CUDA(cudaGetDevice(&dev));
+    CtxLease lease;
+    if (int rc = lease.acquire(dev)) return rc;
+    DeviceCtx &c = *lease.c;
+    void *d = nullptr;
+    AB_CUDA(cudaMallocAsync(&d, bytes, c.st));
+    int rc = 0;
+    cudaEvent_t ev = nullptr;
+    cudaError_t e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventRecord(ev, c.st);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(c.copy_st, ev, 0);
+    if (e != cudaSuccess) rc = cuda_fail(e, "event setup", __FILE__, __LINE__);
+    if (!rc) rc = h2d(c, d, points, bytes);
+    if (!rc) { e = cudaEventRecord(ev, c.copy_st); if (e == cudaSuccess) e = cudaStreamWaitEvent(c.st, ev, 0); if (e != cudaSuccess) rc = cuda_fail(e, "event", __FILE__, __LINE__); }
+    if (!rc) rc = point_ntt_dispatch(curve, d, log_n, inverse, coset_offset, c.st);
+    if (!rc) { e = cudaMemcpyAsync(points, d, bytes, cudaMemcpyDeviceToHost, c.st); if (e != cudaSuccess) rc = cuda_fail(e, "cudaMemcpyAsync D2H", __FILE__, __LINE__); }
+    cudaStreamSynchronize(c.copy_st);
+    cudaFreeAsync(d, c.st);
+    e = cudaStreamSynchronize(c.st);
+    if (!rc && e != cudaSuccess) rc = cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
+    if (ev) cudaEventDestroy(ev);
+    return rc;
 }
 int b200_clear_cache(void) {
     int rc = ntt_clear_cache();

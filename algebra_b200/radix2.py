@@ -3,7 +3,10 @@
 Field elements are (4,) uint64 Montgomery limb arrays, vectors are (n, 4) arrays — numpy on the host path, or
 torch CUDA tensors (8-byte dtype) for device-resident data.  The transforms have the reference's semantics:
   fft_in_place / fft  : input shorter than the domain is zero-padded, longer is TRUNCATED (`coeffs.resize`, :144)
-  ifft_in_place / ifft: same resize (:151); natural order in and out."""
+  ifft_in_place / ifft: same resize (:151); natural order in and out.
+With `curve=` (a B200_CURVE_* id whose scalar field is the domain's field) the coefficients are G1 points instead, the
+T = Projective case of the reference's `DomainCoeff` transforms: (len, 3N) uint64 Jacobian Montgomery limbs (x, y, z), padded
+with the identity (R, R, 0) or truncated to the domain size; every identity in the output is (R, R, 0)."""
 from __future__ import annotations
 
 import ctypes
@@ -11,7 +14,7 @@ import ctypes
 import numpy as np
 
 from . import _lib
-from .params import SCALAR_FIELDS, PrimeField
+from .params import CURVES, SCALAR_FIELDS, PrimeField
 
 
 def _is_torch(x) -> bool:
@@ -133,8 +136,60 @@ class Radix2EvaluationDomain:
         del keep
         return out
 
-    def fft(self, coeffs):
+    # -- G1 point coefficients (T = Projective) ----------------------------------------------------
+    def _point_width(self, curve: int) -> int:
+        if curve not in CURVES or CURVES[curve].ntt_field_id != self.field_id:
+            raise ValueError(f"curve {curve} does not have this domain's scalar field ({self.F.name})")
+        return 3 * CURVES[curve].N
+
+    def _resize_points(self, x, curve: int):
+        w, n = self._point_width(curve), self.size
+        zero = np.zeros(w, dtype=np.uint64)   # Projective::zero() = (1, 1, 0) in Montgomery form (group.rs:142-158)
+        one = CURVES[curve].fq.to_limbs(1)
+        zero[:len(one)] = one
+        zero[w // 3:w // 3 + len(one)] = one
+        if _is_torch(x):
+            import torch
+            x = x.reshape(-1, w)
+            if x.shape[0] == n:
+                return x
+            out = torch.from_numpy(np.tile(zero, (n, 1)).view(np.int64)).to(device=x.device, dtype=x.dtype)
+            k = min(n, x.shape[0])
+            out[:k] = x[:k]
+            return out
+        x = np.asarray(x, dtype=np.uint64).reshape(-1, w)
+        if x.shape[0] == n and x.flags["C_CONTIGUOUS"]:
+            return x
+        out = np.tile(zero, (n, 1))
+        k = min(n, x.shape[0])
+        out[:k] = x[:k]
+        return out
+
+    def _run_points(self, x, inverse: bool, curve: int):
+        keep, offp = self._offset_ptr()
+        if _is_torch(x):
+            import torch
+            if not x.is_cuda or not x.is_contiguous():
+                raise TypeError("device path needs a contiguous CUDA tensor")
+            with torch.cuda.device(x.device):
+                st = torch.cuda.current_stream().cuda_stream
+                _lib.check(_lib.lib().b200_ntt_g1_dev(curve, x.data_ptr(), self.log_size_of_group, int(inverse), offp, st))
+        else:
+            assert x.flags["C_CONTIGUOUS"] and x.dtype == np.uint64
+            _lib.check(_lib.lib().b200_ntt_g1(curve, x.ctypes.data_as(ctypes.c_void_p), self.log_size_of_group, int(inverse), offp))
+        del keep
+        return x
+
+    def _run_points_copy(self, pts, inverse: bool, curve: int):
+        x = self._resize_points(pts, curve)
+        if self._shares(x, pts):
+            x = x.clone() if _is_torch(x) else x.copy()
+        return self._run_points(x, inverse, curve)
+
+    def fft(self, coeffs, curve: int | None = None):
         """EvaluationDomain::fft (poly/src/domain/mod.rs:94-98): returns a new vector of `size` evaluations."""
+        if curve is not None:
+            return self._run_points_copy(coeffs, False, curve)
         if not _is_torch(coeffs):
             return self._run_padded(coeffs, False)
         x = self._resize(coeffs)
@@ -142,7 +197,9 @@ class Radix2EvaluationDomain:
             x = x.clone() if _is_torch(x) else x.copy()
         return self._run(x, False)
 
-    def ifft(self, evals):
+    def ifft(self, evals, curve: int | None = None):
+        if curve is not None:
+            return self._run_points_copy(evals, True, curve)
         if not _is_torch(evals):
             return self._run_padded(evals, True)
         x = self._resize(evals)
@@ -150,12 +207,16 @@ class Radix2EvaluationDomain:
             x = x.clone() if _is_torch(x) else x.copy()
         return self._run(x, True)
 
-    def fft_in_place(self, coeffs):
+    def fft_in_place(self, coeffs, curve: int | None = None):
         """Transforms `coeffs` itself when it already has `size` rows (the Vec is resized otherwise, and the new
         vector is returned — Python cannot grow the caller's buffer in place)."""
+        if curve is not None:
+            return self._run_points(self._resize_points(coeffs, curve), False, curve)
         return self._run(self._resize(coeffs), False)
 
-    def ifft_in_place(self, evals):
+    def ifft_in_place(self, evals, curve: int | None = None):
+        if curve is not None:
+            return self._run_points(self._resize_points(evals, curve), True, curve)
         return self._run(self._resize(evals), True)
 
     def __eq__(self, o):

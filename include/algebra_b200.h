@@ -151,6 +151,21 @@ int b200_ntt_fr_padded(int field, const uint64_t *in, size_t len_in, uint64_t *o
 /* device-resident variant: d_data is a device pointer; coset_offset stays a host pointer. */
 int b200_ntt_fr_dev(int field, void *d_data, uint32_t log_n, int inverse, const uint64_t *coset_offset,
                     void *stream);
+/* FFT over G1 points — Radix2EvaluationDomain::{fft_in_place, ifft_in_place} with T = Projective<g1::Config>
+ * (T: DomainCoeff<Fr>, poly/src/domain/mod.rs:332-361) after the resize step: the same transform as b200_ntt_fr with the
+ * scalars replaced by points,
+ *   forward: out[i] = sum_j (h * g^i)^j * P_j          inverse: the exact inverse incl. 1/n,
+ * over the domain of the curve's scalar field Fr (B200_CURVE_BLS12_381 -> B200_FIELD_BLS12_381_FR, B200_CURVE_BN254 ->
+ * B200_FIELD_BN254_FR: the same number).
+ *   points        2^log_n x 3N u64 (Jacobian x, y, z, Montgomery), transformed in place; any point with z = 0 is the identity,
+ *                 and every identity in the output is written as (R, R, 0)
+ *   coset_offset  NULL (h = 1) or 4 u64 Montgomery limbs of h
+ * Outputs are the reference's group elements; their Jacobian limbs may differ (compare after into_affine).
+ * B200_ETOOLARGE past TWO_ADICITY, B200_EINVAL for a null pointer, an unknown curve or B200_CURVE_BLS12_381_G2 (no launch).
+ * The host entry stages through pinned buffers (pinned or pageable `points`); the _dev entry takes a device pointer and is
+ * ordered on `stream` (coset_offset stays a host pointer). */
+int b200_ntt_g1(int curve, uint64_t *points, uint32_t log_n, int inverse, const uint64_t *coset_offset);
+int b200_ntt_g1_dev(int curve, void *d_points, uint32_t log_n, int inverse, const uint64_t *coset_offset, void *stream);
 /* Dense polynomial product over the scalar field, device-resident end to end: the body of
  * `impl Mul<&DensePolynomial<F>> for &DensePolynomial<F>` (poly/src/polynomial/univariate/dense.rs:641-656) —
  * domain of size n = next_pow2(la + lb - 1), fft(a), fft(b), `self_evals *= &other_evals`

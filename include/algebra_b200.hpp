@@ -22,11 +22,13 @@ namespace ab200 {
 
 struct Bls12_381G1 {
     static constexpr int ID = B200_CURVE_BLS12_381, N = 6;
+    using BaseParams = BlsFq;
     using ScalarParams = BlsFr;
     static constexpr int FIELD_ID = B200_FIELD_BLS12_381_FR;
 };
 struct Bn254G1 {
     static constexpr int ID = B200_CURVE_BN254, N = 4;
+    using BaseParams = BnFq;
     using ScalarParams = BnFr;
     static constexpr int FIELD_ID = B200_FIELD_BN254_FR;
 };
@@ -34,6 +36,7 @@ struct Bn254G1 {
 // G2 of BLS12-381: coordinates in Fq2 = (c0, c1), 12 u64 per coordinate (curves/bls12_381/src/curves/g2.rs:54)
 struct Bls12_381G2 {
     static constexpr int ID = B200_CURVE_BLS12_381_G2, N = 12;
+    using BaseParams = BlsFq;   // Fq2 one = (Fq one, 0)
     using ScalarParams = BlsFr;
     static constexpr int FIELD_ID = B200_FIELD_BLS12_381_FR;
 };
@@ -203,8 +206,26 @@ template <class Curve> class Radix2EvaluationDomain {
     void ifft_in_place(std::vector<Fr> &evals) const { run(evals, 1); }
     std::vector<Fr> fft(std::vector<Fr> coeffs) const { run(coeffs, 0); return coeffs; }
     std::vector<Fr> ifft(std::vector<Fr> evals) const { run(evals, 1); return evals; }
+    // T = Projective<Curve> (G1 point coefficients, DomainCoeff for Projective, poly/src/domain/mod.rs:332-361): resized with
+    // the identity, transformed by b200_ntt_g1; G2 is refused with B200_EINVAL
+    void fft_in_place(std::vector<Projective<Curve>> &coeffs) const { run_points(coeffs, 0); }
+    void ifft_in_place(std::vector<Projective<Curve>> &evals) const { run_points(evals, 1); }
+    std::vector<Projective<Curve>> fft(std::vector<Projective<Curve>> coeffs) const { run_points(coeffs, 0); return coeffs; }
+    std::vector<Projective<Curve>> ifft(std::vector<Projective<Curve>> evals) const { run_points(evals, 1); return evals; }
 
   private:
+    static Projective<Curve> point_zero() {   // Projective::zero() = (1, 1, 0), Montgomery (group.rs:142-158)
+        using PB = typename Curve::BaseParams;
+        Projective<Curve> p{};
+        uint32_t one[PB::L];
+        Fp<PB>::set_one(one);
+        for (int i = 0; i < PB::L / 2; i++) p.x[i] = p.y[i] = (uint64_t)one[2 * i] | ((uint64_t)one[2 * i + 1] << 32);
+        return p;
+    }
+    void run_points(std::vector<Projective<Curve>> &v, int inverse) const {
+        v.resize(size, point_zero());
+        check(b200_ntt_g1(Curve::ID, reinterpret_cast<uint64_t *>(v.data()), log_size_of_group, inverse, offset_is_one() ? nullptr : offset.data()));
+    }
     void run(std::vector<Fr> &v, int inverse) const {
         v.resize(size, Fr{0, 0, 0, 0});
         check(b200_ntt_fr(Curve::FIELD_ID, reinterpret_cast<uint64_t *>(v.data()), log_size_of_group, inverse,

@@ -30,6 +30,9 @@ extern "C" {
     pub fn b200_msm_stream_finish(stream: *mut b200_msm_stream_t, out_xyz: *mut u64) -> c_int;
     pub fn b200_msm_stream_abort(stream: *mut b200_msm_stream_t) -> c_int;
     pub fn b200_ntt_fr(field: c_int, data: *mut u64, log_n: u32, inverse: c_int, coset_offset: *const u64) -> c_int;
+    pub fn b200_ntt_g1(curve: c_int, points: *mut u64, log_n: u32, inverse: c_int, coset_offset: *const u64) -> c_int;
+    pub fn b200_ntt_g1_dev(curve: c_int, d_points: *mut c_void, log_n: u32, inverse: c_int, coset_offset: *const u64,
+                           stream: *mut c_void) -> c_int;
     pub fn b200_g1_sum(curve: c_int, points_xyz: *const u64, k: usize, out_xyz: *mut u64) -> c_int;
 }
 

@@ -9,8 +9,9 @@
 //!   serializes exactly like `Affine<C>`.  The MSM uses every GPU of the node (`b200_msm_sw_g1_multi`).
 //! * NTT — `B200Radix2Domain<F>` wraps `Radix2EvaluationDomain<F>` and implements `EvaluationDomain<F>`
 //!   (poly/src/domain/mod.rs:31-329); `fft_in_place` / `ifft_in_place` resize exactly like radix2/mod.rs:140-153,
-//!   then hand the limb slice to the GPU when `T == F`, and fall back to the inner CPU domain for any other
-//!   `DomainCoeff` (e.g. FFTs over group elements, poly/src/test.rs:57).
+//!   then hand the limb slice to the GPU when `T == F` (`b200_ntt_fr`) or when `T` is G1 `Projective` of BLS12-381 or BN254
+//!   (or of `B200<..>` of them) whose scalar field is `F` (`b200_ntt_g1`, FFTs over group elements as in poly/src/test.rs:57,
+//!   e.g. an SRS to its Lagrange basis), and fall back to the inner CPU domain for any other `DomainCoeff` (G2 included).
 //!
 //! Data crosses the FFI as arkworks' in-memory Montgomery limbs (no serialization): `Fp<MontBackend<_,N>,N>` is
 //! `BigInt<N>([u64; N])` + a ZST, `Affine<P>` is `{x, y, infinity: ()}` with the identity stored as (0,0).
@@ -158,18 +159,51 @@ pub struct B200Radix2Domain<F: B200FftField>(pub Radix2EvaluationDomain<F>);
 
 impl<F: B200FftField> B200Radix2Domain<F> {
     fn gpu<T: DomainCoeff<F>>(&self, x: &mut [T], inverse: bool) -> bool {
-        // Rust has no specialisation and T is not 'static: compare type names + sizes to detect T == F.
-        if core::any::type_name::<T>() != core::any::type_name::<F>() || core::mem::size_of::<T>() != 32 {
-            return false;
-        }
         let off = self.0.coset_offset();
         let offp = if off.is_one() { core::ptr::null() } else { &off as *const F as *const u64 };
-        let rc = unsafe {
-            ffi::b200_ntt_fr(F::FIELD_ID, x.as_mut_ptr() as *mut u64, self.0.log_size_of_group, inverse as i32, offp)
+        // Rust has no specialisation and T is not 'static: compare type names + sizes to detect T == F or a G1 point type.
+        let rc = if core::any::type_name::<T>() == core::any::type_name::<F>() && core::mem::size_of::<T>() == 32 {
+            unsafe { ffi::b200_ntt_fr(F::FIELD_ID, x.as_mut_ptr() as *mut u64, self.0.log_size_of_group, inverse as i32, offp) }
+        } else if let Some(curve) = g1_point_curve::<F, T>() {
+            unsafe { ffi::b200_ntt_g1(curve, x.as_mut_ptr() as *mut u64, self.0.log_size_of_group, inverse as i32, offp) }
+        } else {
+            return false;
         };
         ffi::check(rc);
         true
     }
+}
+
+/// The curve id when `T` is `Projective` of a G1 the library has point-FFT kernels for (directly or through `B200<..>`) and its
+/// scalar field is `F`; the point layout (x, y, z, each N Montgomery limbs) is asserted before the slice is handed over.
+fn g1_point_curve<F: B200FftField, T>() -> Option<core::ffi::c_int> {
+    fn is<C: B200Curve, F: B200FftField, T>() -> bool {
+        use core::any::type_name;
+        let named = type_name::<T>() == type_name::<Projective<C>>() || type_name::<T>() == type_name::<Projective<B200<C>>>();
+        if !named || type_name::<C::ScalarField>() != type_name::<F>() {
+            return false;
+        }
+        projective_layout_checks::<C>();
+        core::mem::size_of::<T>() == 24 * C::N
+    }
+    if is::<ark_bls12_381::g1::Config, F, T>() {
+        Some(ffi::B200_CURVE_BLS12_381)
+    } else if is::<ark_bn254::g1::Config, F, T>() {
+        Some(ffi::B200_CURVE_BN254)
+    } else {
+        None
+    }
+}
+
+fn projective_layout_checks<C: B200Curve>() {
+    use core::mem::size_of;
+    assert_eq!(size_of::<Projective<C>>(), 24 * C::N);
+    assert_eq!(size_of::<Projective<B200<C>>>(), 24 * C::N);
+    let probe = Projective::<C>::default();
+    let base = &probe as *const _ as usize;
+    assert_eq!(&probe.x as *const _ as usize - base, 0, "Projective.x must be at offset 0");
+    assert_eq!(&probe.y as *const _ as usize - base, 8 * C::N, "Projective.y must follow x");
+    assert_eq!(&probe.z as *const _ as usize - base, 16 * C::N, "Projective.z must follow y");
 }
 
 impl<F: B200FftField> EvaluationDomain<F> for B200Radix2Domain<F> {
