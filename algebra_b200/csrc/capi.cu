@@ -7,43 +7,9 @@
 #include <thread>
 #include <vector>
 #include "common.cuh"
+#include "host_api.h"
 
 namespace ab200 {
-int ntt_dispatch(int field, void *d_data, uint32_t log_n, int inverse, const uint64_t *coset, cudaStream_t st);
-int ntt_clear_cache();
-int point_ntt_check(int curve, const void *points, uint32_t log_n);
-int point_ntt_coord_words(int curve);
-int point_ntt_dispatch(int curve, void *d_points, uint32_t log_n, int inverse, const uint64_t *coset, cudaStream_t st);
-struct MsmSessionBase {
-    virtual ~MsmSessionBase() {}
-    virtual int begin(size_t n_total, size_t max_chunk, int kind, cudaStream_t st) = 0;
-    virtual int add_chunk(const void *d_bases, const void *d_scalars, size_t nk, cudaEvent_t ready) = 0;
-    virtual int finish(void *d_out) = 0;
-    virtual int collect_timings() = 0;
-    virtual int coord_words() const = 0;
-};
-MsmSessionBase *msm_session_create(int curve);
-int msm_coord_words(int curve);
-void msm_write_zero(int curve, uint64_t *out_xyz);
-int msm_dispatch(int curve, int kind, const void *d_bases, const void *d_scalars, size_t n, uint64_t *out_xyz_host, cudaStream_t st, int K,
-                 const size_t *chunk_off, const cudaEvent_t *ready);
-size_t scalar_kind_bytes(int kind);
-int msm_set_window(int c);
-int msm_set_affine_levels(int levels);
-int msm_get_window();
-int msm_get_affine_levels();
-int msm_set_bucket_slice(int slice, int slices);
-void msm_get_bucket_slice(int *slice, int *slices);
-int msm_auto_window(size_t n, int scalar_bits);
-int msm_last_timings(float *ms7, int *c, int *windows, unsigned long long *bucket_adds);
-int g1_sum_dispatch(int curve, const uint64_t *pts_host, size_t k, uint64_t *out_host, bool to_affine);
-int fp_op_dispatch(int field, int op, const void *a, const void *b, void *out, size_t n, int reps, cudaStream_t st);
-int ec_op_dispatch(int curve, int op, const void *a, const void *b, void *out, size_t n, cudaStream_t st);
-int gen_bases_dispatch(int curve, uint64_t seed, size_t n, void *d_bases, void *d_b, cudaStream_t st);
-int gen_scalars_dispatch(int field, uint64_t seed, size_t n, void *d_scalars, cudaStream_t st);
-int batch_mul_dispatch(int curve, const uint64_t *base_xy, const void *d_scalars, size_t n, void *d_out, cudaStream_t st);
-int normalize_batch_dispatch(int curve, const void *d_xyz, size_t n, void *d_out, cudaStream_t st);
-
 // ------------------------------------------------------------------------------------------------
 // Host-buffer plumbing: per-device contexts (compute stream, copy stream, pinned staging ring), leased per call so that
 // concurrent callers and the per-device worker threads of the multi-GPU entry points never share one.
@@ -137,6 +103,79 @@ static int h2d(DeviceCtx &c, void *dst, const void *src, size_t bytes) {
     return 0;
 }
 
+// One call with host buffers on the CURRENT device: the leased context `c`, the call's stream-ordered scratch and its events.
+// Uploads run on c->copy_st, the compute and the downloads on c->st.  On every exit path the destructor synchronises both
+// streams before it frees anything: nothing of the call is in flight when it returns, and the caller may reuse its buffers.
+struct HostCall {
+    CtxLease lease;
+    DeviceCtx *c = nullptr;
+    std::vector<void *> mem;
+    std::vector<cudaEvent_t> ev;
+    bool alloc_pending = false;   // scratch allocated on c->st that c->copy_st is not yet ordered after
+
+    int begin() {
+        int dev = 0;
+        AB_CUDA(cudaGetDevice(&dev));
+        if (int rc = lease.acquire(dev)) return rc;
+        c = lease.c;
+        return 0;
+    }
+    template <class T> int alloc(T **p, size_t bytes) {
+        void *q = nullptr;
+        AB_CUDA(cudaMallocAsync(&q, bytes ? bytes : 16, c->st));
+        mem.push_back(q);
+        *p = (T *)q;
+        alloc_pending = true;
+        return 0;
+    }
+    // device dst <- host src through h2d, after the scratch allocated so far
+    int upload(void *dst, const void *src, size_t bytes) {
+        if (alloc_pending) {
+            cudaEvent_t e;
+            if (int rc = event(&e)) return rc;
+            AB_CUDA(cudaEventRecord(e, c->st));
+            AB_CUDA(cudaStreamWaitEvent(c->copy_st, e, 0));
+            alloc_pending = false;
+        }
+        return h2d(*c, dst, src, bytes);
+    }
+    // *done fires when every upload so far has landed
+    int uploaded(cudaEvent_t *done) {
+        if (int rc = event(done)) return rc;
+        AB_CUDA(cudaEventRecord(*done, c->copy_st));
+        return 0;
+    }
+    int wait_uploads() {   // c->st waits for every upload so far
+        cudaEvent_t done;
+        if (int rc = uploaded(&done)) return rc;
+        AB_CUDA(cudaStreamWaitEvent(c->st, done, 0));
+        return 0;
+    }
+    int download(void *dst, const void *src, size_t bytes) {
+        cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->st);
+        return e == cudaSuccess ? 0 : cuda_fail(e, "cudaMemcpyAsync D2H", __FILE__, __LINE__);
+    }
+    int sync() {   // the result of a successful call is on the host
+        cudaError_t e = cudaStreamSynchronize(c->st);
+        return e == cudaSuccess ? 0 : cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
+    }
+    ~HostCall() {
+        if (!c) return;
+        cudaStreamSynchronize(c->copy_st);
+        cudaStreamSynchronize(c->st);
+        for (void *p : mem) cudaFreeAsync(p, c->st);
+        for (cudaEvent_t e : ev) cudaEventDestroy(e);
+        cudaStreamSynchronize(c->st);
+    }
+
+private:
+    int event(cudaEvent_t *e) {
+        AB_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+        ev.push_back(*e);
+        return 0;
+    }
+};
+
 // chunk boundaries of the host path in 16ths of n.  Growing chunks: only the first, small transfer is exposed and every later
 // one is shorter than the arithmetic of the chunk before it; few chunks, because small chunks run the accumulation less
 // efficiently (short bucket runs) and each extra chunk costs a bucket-merge pass.  B200_MSM_CHUNKS="2,8,16" overrides (read once).
@@ -166,14 +205,10 @@ static const ChunkPlan &chunk_plan() {
 // The whole host-buffer MSM on the CURRENT device: allocate, pipeline (H2D chunk k+1 | sort + accumulate chunk k), reduce,
 // D2H.  `d_bases_resident` != null: the bases already live on this device and only the scalars travel.
 static int host_msm(int curve, int kind, const void *bases, const void *d_bases_resident, const void *scalars, size_t n, uint64_t *out_xyz) {
-    const int L = msm_coord_words(curve);
     if (n == 0) { msm_write_zero(curve, out_xyz); return 0; }
-    int dev = 0;
-    AB_CUDA(cudaGetDevice(&dev));
-    CtxLease lease;
-    if (int rc = lease.acquire(dev)) return rc;
-    DeviceCtx &c = *lease.c;
-    const size_t sb = scalar_kind_bytes(kind), pb = (size_t)2 * L * 4;
+    HostCall h;
+    if (int rc = h.begin()) return rc;
+    const size_t sb = scalar_kind_bytes(kind), pb = (size_t)2 * curve_info(curve)->coord_words * 4;
     const ChunkPlan &plan = chunk_plan();
     const int K = n >= ((size_t)1 << 22) ? plan.K : 1;
     size_t off[9];
@@ -182,50 +217,28 @@ static int host_msm(int curve, int kind, const void *bases, const void *d_bases_
     size_t max_chunk = 0;
     for (int k = 0; k < K; k++) max_chunk = std::max(max_chunk, off[k + 1] - off[k]);
 
-    struct Cleanup {   // every exit path: nothing in flight, nothing leaked
-        DeviceCtx &c;
-        void *d_bases = nullptr, *d_scalars = nullptr, *d_out = nullptr;
-        std::vector<cudaEvent_t> ev;
-        ~Cleanup() {
-            cudaStreamSynchronize(c.copy_st);
-            cudaStreamSynchronize(c.st);
-            for (void *p : {d_bases, d_scalars, d_out})
-                if (p) cudaFreeAsync(p, c.st);
-            for (auto e : ev) cudaEventDestroy(e);
-            cudaStreamSynchronize(c.st);
-        }
-    } cl{c};
-    std::unique_ptr<MsmSessionBase> s(msm_session_create(curve));   // destroyed BEFORE cl: its frees are enqueued on c.st, then cl syncs
-    cudaEvent_t alloc_done;
-    AB_CUDA(cudaEventCreateWithFlags(&alloc_done, cudaEventDisableTiming));
-    cl.ev.push_back(alloc_done);
-    if (!d_bases_resident) AB_CUDA(cudaMallocAsync(&cl.d_bases, n * pb, c.st));
-    AB_CUDA(cudaMallocAsync(&cl.d_scalars, n * sb, c.st));
-    AB_CUDA(cudaMallocAsync(&cl.d_out, (size_t)3 * L * 4, c.st));
-    AB_CUDA(cudaEventRecord(alloc_done, c.st));
-    AB_CUDA(cudaStreamWaitEvent(c.copy_st, alloc_done, 0));
-    const char *db = d_bases_resident ? (const char *)d_bases_resident : (const char *)cl.d_bases;
-    if (int rc = s->begin(n, max_chunk, kind, c.st)) return rc;
+    std::unique_ptr<MsmSessionBase> s(msm_session_create(curve));   // destroyed BEFORE h: its frees are enqueued on c->st, then h syncs
+    char *d_bases = nullptr, *d_scalars = nullptr;
+    if (!d_bases_resident)
+        if (int rc = h.alloc(&d_bases, n * pb)) return rc;
+    if (int rc = h.alloc(&d_scalars, n * sb)) return rc;
+    const char *db = d_bases_resident ? (const char *)d_bases_resident : d_bases;
+    if (int rc = s->begin(n, max_chunk, kind, h.c->st)) return rc;
     for (int k = 0; k < K; k++) {
         const size_t lo = off[k], cnt = off[k + 1] - off[k];
-        cudaEvent_t ready;
-        AB_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
-        cl.ev.push_back(ready);
-        if (int rc = h2d(c, (char *)cl.d_scalars + lo * sb, (const char *)scalars + lo * sb, cnt * sb)) return rc;
+        if (int rc = h.upload(d_scalars + lo * sb, (const char *)scalars + lo * sb, cnt * sb)) return rc;
         if (!d_bases_resident)
-            if (int rc = h2d(c, (char *)cl.d_bases + lo * pb, (const char *)bases + lo * pb, cnt * pb)) return rc;
-        AB_CUDA(cudaEventRecord(ready, c.copy_st));
-        if (int rc = s->add_chunk(db + lo * pb, (const char *)cl.d_scalars + lo * sb, cnt, ready)) return rc;
+            if (int rc = h.upload(d_bases + lo * pb, (const char *)bases + lo * pb, cnt * pb)) return rc;
+        cudaEvent_t ready;
+        if (int rc = h.uploaded(&ready)) return rc;
+        if (int rc = s->add_chunk(db + lo * pb, d_scalars + lo * sb, cnt, ready)) return rc;
     }
-    if (int rc = s->finish(cl.d_out)) return rc;
-    AB_CUDA(cudaMemcpyAsync(out_xyz, cl.d_out, (size_t)3 * L * 4, cudaMemcpyDeviceToHost, c.st));
-    AB_CUDA(cudaStreamSynchronize(c.st));
-    return s->collect_timings();
+    return msm_session_result(*s, out_xyz, h.c->st);
 }
 
 static int check_msm_args(int curve, int kind, const void *bases, const void *scalars, size_t n, const void *out) {
-    if (kind < B200_SCALARS_FR_MONT || kind > B200_SCALARS_U64) { set_last_error("unknown scalar kind"); return B200_EINVAL; }
-    if (!msm_coord_words(curve)) { set_last_error("unknown curve id"); return B200_EINVAL; }
+    if (int rc = check_scalar_kind(kind)) return rc;
+    if (!curve_info(curve)) { set_last_error("unknown curve id"); return B200_EINVAL; }
     if (!out || (n && (!bases || !scalars))) { set_last_error("null pointer"); return B200_EINVAL; }
     if (n >= ((size_t)1 << 31)) { set_last_error("n must be < 2^31 per device"); return B200_ETOOLARGE; }
     return 0;
@@ -267,6 +280,42 @@ template <class Fn> static int per_device(int ngpus, Fn fn) {
     cudaSetDevice(dev0);
     for (int d = 0; d < ngpus; d++)
         if (rc[d]) { set_last_error("device " + std::to_string(d) + ": " + msg[d]); return rc[d]; }
+    return 0;
+}
+
+// host points in, host result out: the sum of k Jacobian points, or (to_affine) the affine form of each of the k points
+static int host_g1_sum(int curve, const uint64_t *pts, size_t k, uint64_t *out, bool to_affine) {
+    const CurveInfo *ci = curve_info(curve);
+    if (!ci) { set_last_error("unknown curve id"); return B200_EINVAL; }
+    if (!pts || !out) { set_last_error("null pointer"); return B200_EINVAL; }
+    const size_t L = (size_t)ci->coord_words, in_bytes = k * 3 * L * 4, out_bytes = (to_affine ? k * 2 * L : 3 * L) * 4;
+    HostCall h;
+    void *d_in = nullptr, *d_out = nullptr;
+    if (int rc = h.begin()) return rc;
+    if (int rc = h.alloc(&d_in, in_bytes)) return rc;
+    if (int rc = h.alloc(&d_out, out_bytes)) return rc;
+    if (int rc = h.upload(d_in, pts, in_bytes)) return rc;
+    if (int rc = h.wait_uploads()) return rc;
+    if (int rc = g1_sum(curve, d_in, k, d_out, to_affine, h.c->st)) return rc;
+    if (int rc = h.download(out, d_out, out_bytes)) return rc;
+    return h.sync();
+}
+
+// one MSM split over ngpus devices: part(d, partial) computes device d's Jacobian result into `partial`; the partial results
+// are then added on the current device
+template <class Fn> static int msm_over_devices(int curve, int ngpus, uint64_t *out_xyz, Fn part) {
+    const size_t words = (size_t)3 * curve_info(curve)->coord_words / 2;   // u64 per Jacobian point
+    std::vector<uint64_t> partial((size_t)ngpus * words);
+    if (int rc = per_device(ngpus, [&](int d) { return part(d, partial.data() + (size_t)d * words); })) return rc;
+    if (ngpus == 1) { memcpy(out_xyz, partial.data(), words * 8); return 0; }
+    return host_g1_sum(curve, partial.data(), (size_t)ngpus, out_xyz, false);
+}
+
+// the device-buffer entry points: dispatch(st) on the caller's stream, then wait for it
+template <class Fn> static int on_stream(void *stream, Fn dispatch) {
+    if (int rc = ensure_device_init()) return rc;
+    if (int rc = dispatch((cudaStream_t)stream)) return rc;
+    AB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
     return 0;
 }
 }  // namespace ab200
@@ -320,29 +369,24 @@ int b200_device_count(void) {
 int b200_msm_sw_g1_multi(int curve, int ngpus, const uint64_t *bases, const uint64_t *scalars, size_t n, uint64_t *out_xyz) {
     if (int rc = check_msm_args(curve, B200_SCALARS_FR_MONT, bases, scalars, n / std::max(ngpus, 1), out_xyz)) return rc;
     if (ngpus < 1 || ngpus > b200_device_count()) { set_last_error("ngpus must be in [1, b200_device_count()]"); return B200_EINVAL; }
-    const int L = msm_coord_words(curve);
     if (n == 0) { msm_write_zero(curve, out_xyz); return 0; }
-    std::vector<uint64_t> partial((size_t)ngpus * 3 * L / 2);
-    int rc = per_device(ngpus, [&](int d) {
+    const size_t pb = (size_t)2 * curve_info(curve)->coord_words * 4;
+    return msm_over_devices(curve, ngpus, out_xyz, [&](int d, uint64_t *partial) {
         size_t lo, hi;
         shard(n, ngpus, d, &lo, &hi);
-        return host_msm(curve, B200_SCALARS_FR_MONT, (const char *)bases + lo * (size_t)(2 * L * 4), nullptr, (const char *)scalars + lo * 32, hi - lo,
-                        partial.data() + (size_t)d * 3 * L / 2);
+        return host_msm(curve, B200_SCALARS_FR_MONT, (const char *)bases + lo * pb, nullptr, (const char *)scalars + lo * 32, hi - lo, partial);
     });
-    if (rc) return rc;
-    if (ngpus == 1) { memcpy(out_xyz, partial.data(), (size_t)3 * L * 4); return 0; }
-    return g1_sum_dispatch(curve, partial.data(), (size_t)ngpus, out_xyz, false);
 }
 
 int b200_bases_upload(int curve, int ngpus, const uint64_t *bases, size_t n, b200_bases_t **handle) {
-    const int L = msm_coord_words(curve);
-    if (!L) { set_last_error("unknown curve id"); return B200_EINVAL; }
+    const CurveInfo *ci = curve_info(curve);
+    if (!ci) { set_last_error("unknown curve id"); return B200_EINVAL; }
     if (!handle || (n && !bases)) { set_last_error("null pointer"); return B200_EINVAL; }
     if (ngpus < 1 || ngpus > b200_device_count()) { set_last_error("ngpus must be in [1, b200_device_count()]"); return B200_EINVAL; }
     std::unique_ptr<b200_bases> h(new b200_bases());
     h->curve = curve; h->ngpus = ngpus; h->n = n;
     h->d_ptr.assign((size_t)ngpus, nullptr); h->lo.resize((size_t)ngpus); h->hi.resize((size_t)ngpus);
-    const size_t pb = (size_t)2 * L * 4;
+    const size_t pb = (size_t)2 * ci->coord_words * 4;
     int rc = per_device(ngpus, [&](int d) {
         shard(n, ngpus, d, &h->lo[d], &h->hi[d]);
         const size_t cnt = h->hi[d] - h->lo[d];
@@ -373,25 +417,20 @@ int b200_msm_bases(const b200_bases_t *h, int scalar_kind, const void *scalars, 
     if (!h) { set_last_error("null handle"); return B200_EINVAL; }
     if (n > h->n) { set_last_error("more scalars than uploaded bases"); return B200_EINVAL; }
     if (int rc = check_msm_args(h->curve, scalar_kind, scalars, scalars, n / (size_t)h->ngpus, out_xyz)) return rc;
-    const int L = msm_coord_words(h->curve);
     if (n == 0) { msm_write_zero(h->curve, out_xyz); return 0; }
     const size_t sb = scalar_kind_bytes(scalar_kind);
-    std::vector<uint64_t> partial((size_t)h->ngpus * 3 * L / 2);
-    int rc = per_device(h->ngpus, [&](int d) {
+    return msm_over_devices(h->curve, h->ngpus, out_xyz, [&](int d, uint64_t *partial) {
         const size_t lo = std::min(n, h->lo[d]), hi = std::min(n, h->hi[d]);   // the first n bases
-        return host_msm(h->curve, scalar_kind, nullptr, h->d_ptr[d], (const char *)scalars + lo * sb, hi - lo, partial.data() + (size_t)d * 3 * L / 2);
+        return host_msm(h->curve, scalar_kind, nullptr, h->d_ptr[d], (const char *)scalars + lo * sb, hi - lo, partial);
     });
-    if (rc) return rc;
-    if (h->ngpus == 1) { memcpy(out_xyz, partial.data(), (size_t)3 * L * 4); return 0; }
-    return g1_sum_dispatch(h->curve, partial.data(), (size_t)h->ngpus, out_xyz, false);
 }
 
 int b200_msm_stream_begin(int curve, int scalar_kind, size_t n_total_hint, size_t max_chunk, b200_msm_stream_t **stream) {
     { int irc = ensure_device_init(); if (irc) return irc; }
     if (!stream || !max_chunk) { set_last_error("null handle pointer or max_chunk == 0"); return B200_EINVAL; }
-    if (scalar_kind < B200_SCALARS_FR_MONT || scalar_kind > B200_SCALARS_U64) { set_last_error("unknown scalar kind"); return B200_EINVAL; }
-    const int L = msm_coord_words(curve);
-    if (!L) { set_last_error("unknown curve id"); return B200_EINVAL; }
+    if (int rc = check_scalar_kind(scalar_kind)) return rc;
+    const CurveInfo *ci = curve_info(curve);
+    if (!ci) { set_last_error("unknown curve id"); return B200_EINVAL; }
     std::unique_ptr<b200_msm_stream> s(new b200_msm_stream());
     s->curve = curve; s->kind = scalar_kind; s->max_chunk = max_chunk;
     AB_CUDA(cudaGetDevice(&s->dev));
@@ -400,7 +439,7 @@ int b200_msm_stream_begin(int curve, int scalar_kind, size_t n_total_hint, size_
     DeviceCtx &c = *s->lease.c;
     int rc = s->session->begin(std::max(n_total_hint, max_chunk), max_chunk, scalar_kind, c.st);
     for (int i = 0; i < 2 && !rc; i++) {
-        cudaError_t e = cudaMalloc(&s->d_bases[i], max_chunk * (size_t)(2 * L * 4));
+        cudaError_t e = cudaMalloc(&s->d_bases[i], max_chunk * (size_t)(2 * ci->coord_words * 4));
         if (e == cudaSuccess) e = cudaMalloc(&s->d_scalars[i], max_chunk * scalar_kind_bytes(scalar_kind));
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->consumed[i], cudaEventDisableTiming);
         if (e != cudaSuccess) rc = cuda_fail(e, "stream staging allocation", __FILE__, __LINE__);
@@ -418,7 +457,7 @@ int b200_msm_stream_push(b200_msm_stream_t *s, const uint64_t *bases, const void
     AB_CUDA(cudaGetDevice(&dev));
     if (dev != s->dev) AB_CUDA(cudaSetDevice(s->dev));
     DeviceCtx &c = *s->lease.c;
-    const int L = msm_coord_words(s->curve), b = s->pushes & 1;
+    const int L = curve_info(s->curve)->coord_words, b = s->pushes & 1;
     int rc = 0;
     cudaEvent_t ready = nullptr;
     cudaError_t e = cudaStreamWaitEvent(c.copy_st, s->consumed[b], 0);   // staging buffer b was last read by push k-2
@@ -459,18 +498,7 @@ int b200_msm_stream_finish(b200_msm_stream_t *s, uint64_t *out_xyz) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaSetDevice(s->dev);
-    DeviceCtx &c = *s->lease.c;
-    const int L = msm_coord_words(s->curve);
-    void *d_out = nullptr;
-    int rc = 0;
-    cudaError_t e = cudaMallocAsync(&d_out, (size_t)3 * L * 4, c.st);
-    if (e != cudaSuccess) rc = cuda_fail(e, "cudaMallocAsync", __FILE__, __LINE__);
-    if (!rc) rc = s->session->finish(d_out);
-    if (!rc) { e = cudaMemcpyAsync(out_xyz, d_out, (size_t)3 * L * 4, cudaMemcpyDeviceToHost, c.st); if (e != cudaSuccess) rc = cuda_fail(e, "cudaMemcpyAsync D2H", __FILE__, __LINE__); }
-    if (d_out) cudaFreeAsync(d_out, c.st);
-    e = cudaStreamSynchronize(c.st);
-    if (!rc && e != cudaSuccess) rc = cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
-    if (!rc) rc = s->session->collect_timings();
+    const int rc = msm_session_result(*s->session, out_xyz, s->lease.c->st);
     cudaSetDevice(dev);
     b200_msm_stream_abort(s);
     return rc;
@@ -480,18 +508,15 @@ int b200_set_msm_window(int c) { return msm_set_window(c); }
 int b200_set_msm_affine_levels(int levels) { return msm_set_affine_levels(levels); }
 int b200_set_msm_bucket_slice(int slice, int slices) { return msm_set_bucket_slice(slice, slices); }
 int b200_msm_window_for(int curve, size_t n) {
-    if (!msm_coord_words(curve)) return B200_EINVAL;
-    return msm_auto_window(n, curve == B200_CURVE_BN254 ? 254 : 255);
+    const CurveInfo *ci = curve_info(curve);
+    if (!ci) return B200_EINVAL;
+    return msm_auto_window(n, ci->scalar_bits);
 }
-int b200_g1_sum(int curve, const uint64_t *points_xyz, size_t k, uint64_t *out_xyz) { if (int irc = ensure_device_init()) return irc; return g1_sum_dispatch(curve, points_xyz, k, out_xyz, false); }
-int b200_g1_into_affine(int curve, const uint64_t *xyz, uint64_t *out_xy) { if (int irc = ensure_device_init()) return irc; return g1_sum_dispatch(curve, xyz, 1, out_xy, true); }
+int b200_g1_sum(int curve, const uint64_t *points_xyz, size_t k, uint64_t *out_xyz) { if (int irc = ensure_device_init()) return irc; return host_g1_sum(curve, points_xyz, k, out_xyz, false); }
+int b200_g1_into_affine(int curve, const uint64_t *xyz, uint64_t *out_xy) { if (int irc = ensure_device_init()) return irc; return host_g1_sum(curve, xyz, 1, out_xy, true); }
 
 int b200_ntt_fr_dev(int field, void *d_data, uint32_t log_n, int inverse, const uint64_t *coset_offset, void *stream) {
-    { int irc = ensure_device_init(); if (irc) return irc; }
-    int rc = ntt_dispatch(field, d_data, log_n, inverse, coset_offset, (cudaStream_t)stream);
-    if (rc) return rc;
-    AB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    return 0;
+    return on_stream(stream, [&](cudaStream_t st) { return ntt_dispatch(field, d_data, log_n, inverse, coset_offset, st); });
 }
 
 // host-buffer transform: H2D of the `len_in` given elements only (the zero padding of `fft_in_place`'s resize is produced on the
@@ -499,76 +524,45 @@ int b200_ntt_fr_dev(int field, void *d_data, uint32_t log_n, int inverse, const 
 int b200_ntt_fr_padded(int field, const uint64_t *in, size_t len_in, uint64_t *out, uint32_t log_n, int inverse, const uint64_t *coset_offset) {
     { int irc = ensure_device_init(); if (irc) return irc; }
     if (!out || (len_in && !in)) { set_last_error("null data pointer"); return B200_EINVAL; }
-    if (field != B200_FIELD_BLS12_381_FR && field != B200_FIELD_BN254_FR) { set_last_error("unknown scalar field id"); return B200_EINVAL; }
-    if (log_n > (uint32_t)(field == B200_FIELD_BLS12_381_FR ? 32 : 28)) {
+    const FieldInfo *fi = field_info(field);
+    if (!fi) { set_last_error("unknown scalar field id"); return B200_EINVAL; }
+    if (log_n > (uint32_t)fi->two_adicity) {
         set_last_error("log_n exceeds TWO_ADICITY (Radix2EvaluationDomain::new would return None)");
         return B200_ETOOLARGE;
     }
     const size_t n = (size_t)1 << log_n, bytes = n * 32;
     if (len_in > n) len_in = n;   // coeffs.resize(self.size(), ..) truncates (radix2/mod.rs:144)
-    int dev = 0;
-    AB_CUDA(cudaGetDevice(&dev));
-    CtxLease lease;
-    if (int rc = lease.acquire(dev)) return rc;
-    DeviceCtx &c = *lease.c;
-    void *d = nullptr;
-    AB_CUDA(cudaMallocAsync(&d, bytes, c.st));
-    int rc = 0;
-    cudaEvent_t ev = nullptr;
-    cudaError_t e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventRecord(ev, c.st);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(c.copy_st, ev, 0);
-    if (e != cudaSuccess) rc = cuda_fail(e, "event setup", __FILE__, __LINE__);
-    if (!rc) rc = h2d(c, d, in, len_in * 32);                       // pinned: async; pageable: staged through the pinned ring
-    if (!rc) { e = cudaEventRecord(ev, c.copy_st); if (e == cudaSuccess) e = cudaStreamWaitEvent(c.st, ev, 0); if (e != cudaSuccess) rc = cuda_fail(e, "event", __FILE__, __LINE__); }
-    if (!rc && len_in < n) { e = cudaMemsetAsync((char *)d + len_in * 32, 0, (n - len_in) * 32, c.st); if (e != cudaSuccess) rc = cuda_fail(e, "cudaMemsetAsync", __FILE__, __LINE__); }
-    if (!rc) rc = ntt_dispatch(field, d, log_n, inverse, coset_offset, c.st);
-    if (!rc) { e = cudaMemcpyAsync(out, d, bytes, cudaMemcpyDeviceToHost, c.st); if (e != cudaSuccess) rc = cuda_fail(e, "cudaMemcpyAsync D2H", __FILE__, __LINE__); }
-    cudaStreamSynchronize(c.copy_st);
-    cudaFreeAsync(d, c.st);
-    e = cudaStreamSynchronize(c.st);
-    if (!rc && e != cudaSuccess) rc = cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
-    if (ev) cudaEventDestroy(ev);
-    return rc;
+    HostCall h;
+    char *d = nullptr;
+    if (int rc = h.begin()) return rc;
+    if (int rc = h.alloc(&d, bytes)) return rc;
+    if (int rc = h.upload(d, in, len_in * 32)) return rc;   // in == out (b200_ntt_fr): the D2H below is ordered after this upload
+    if (int rc = h.wait_uploads()) return rc;
+    if (len_in < n) AB_CUDA(cudaMemsetAsync(d + len_in * 32, 0, (n - len_in) * 32, h.c->st));
+    if (int rc = ntt_dispatch(field, d, log_n, inverse, coset_offset, h.c->st)) return rc;
+    if (int rc = h.download(out, d, bytes)) return rc;
+    return h.sync();
 }
 int b200_ntt_fr(int field, uint64_t *data, uint32_t log_n, int inverse, const uint64_t *coset_offset) {
     return b200_ntt_fr_padded(field, data, log_n <= 40 ? (size_t)1 << log_n : 0, data, log_n, inverse, coset_offset);
 }
 int b200_ntt_g1_dev(int curve, void *d_points, uint32_t log_n, int inverse, const uint64_t *coset_offset, void *stream) {
-    { int irc = ensure_device_init(); if (irc) return irc; }
-    int rc = point_ntt_dispatch(curve, d_points, log_n, inverse, coset_offset, (cudaStream_t)stream);
-    if (rc) return rc;
-    AB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    return 0;
+    return on_stream(stream, [&](cudaStream_t st) { return point_ntt_dispatch(curve, d_points, log_n, inverse, coset_offset, st); });
 }
 // host-buffer point transform: staged H2D (pinned or pageable), transform in place on the device, D2H
 int b200_ntt_g1(int curve, uint64_t *points, uint32_t log_n, int inverse, const uint64_t *coset_offset) {
     { int irc = ensure_device_init(); if (irc) return irc; }
     if (int rc = point_ntt_check(curve, points, log_n)) return rc;
-    const size_t bytes = ((size_t)1 << log_n) * 3 * (size_t)point_ntt_coord_words(curve) * 4;
-    int dev = 0;
-    AB_CUDA(cudaGetDevice(&dev));
-    CtxLease lease;
-    if (int rc = lease.acquire(dev)) return rc;
-    DeviceCtx &c = *lease.c;
+    const size_t bytes = ((size_t)1 << log_n) * 3 * (size_t)curve_info(curve)->coord_words * 4;
+    HostCall h;
     void *d = nullptr;
-    AB_CUDA(cudaMallocAsync(&d, bytes, c.st));
-    int rc = 0;
-    cudaEvent_t ev = nullptr;
-    cudaError_t e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventRecord(ev, c.st);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(c.copy_st, ev, 0);
-    if (e != cudaSuccess) rc = cuda_fail(e, "event setup", __FILE__, __LINE__);
-    if (!rc) rc = h2d(c, d, points, bytes);
-    if (!rc) { e = cudaEventRecord(ev, c.copy_st); if (e == cudaSuccess) e = cudaStreamWaitEvent(c.st, ev, 0); if (e != cudaSuccess) rc = cuda_fail(e, "event", __FILE__, __LINE__); }
-    if (!rc) rc = point_ntt_dispatch(curve, d, log_n, inverse, coset_offset, c.st);
-    if (!rc) { e = cudaMemcpyAsync(points, d, bytes, cudaMemcpyDeviceToHost, c.st); if (e != cudaSuccess) rc = cuda_fail(e, "cudaMemcpyAsync D2H", __FILE__, __LINE__); }
-    cudaStreamSynchronize(c.copy_st);
-    cudaFreeAsync(d, c.st);
-    e = cudaStreamSynchronize(c.st);
-    if (!rc && e != cudaSuccess) rc = cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
-    if (ev) cudaEventDestroy(ev);
-    return rc;
+    if (int rc = h.begin()) return rc;
+    if (int rc = h.alloc(&d, bytes)) return rc;
+    if (int rc = h.upload(d, points, bytes)) return rc;
+    if (int rc = h.wait_uploads()) return rc;
+    if (int rc = point_ntt_dispatch(curve, d, log_n, inverse, coset_offset, h.c->st)) return rc;
+    if (int rc = h.download(points, d, bytes)) return rc;
+    return h.sync();
 }
 int b200_clear_cache(void) {
     int rc = ntt_clear_cache();
@@ -584,12 +578,13 @@ int b200_clear_cache(void) {
 }
 
 size_t b200_poly_mul_size(int field, size_t la, size_t lb) {
-    if ((field != B200_FIELD_BLS12_381_FR && field != B200_FIELD_BN254_FR) || la == 0 || lb == 0) return 0;
+    const FieldInfo *fi = field_info(field);
+    if (!fi || la == 0 || lb == 0) return 0;
     const size_t need = la + lb - 1;
     size_t n = 1;
     uint32_t lg = 0;
     while (n < need) { n <<= 1; lg++; }
-    return lg > (uint32_t)(field == B200_FIELD_BLS12_381_FR ? 32 : 28) ? 0 : n;
+    return lg > (uint32_t)fi->two_adicity ? 0 : n;
 }
 
 static int poly_mul_on_device(int field, const void *d_a, size_t la, const void *d_b, size_t lb, void *d_out, cudaStream_t st) {
@@ -607,19 +602,17 @@ static int poly_mul_on_device(int field, const void *d_a, size_t la, const void 
     int rc = ntt_dispatch(field, d_out, lg, 0, nullptr, st);
     if (!rc) rc = ntt_dispatch(field, tmp, lg, 0, nullptr, st);
     // self_evals *= &other_evals ; interpolate
-    if (!rc) rc = fp_op_dispatch(field == B200_FIELD_BLS12_381_FR ? 1 : 3, 0, d_out, tmp, d_out, n, 1, st);
+    if (!rc) rc = fp_op_dispatch(field_info(field)->fp_op_field, 0, d_out, tmp, d_out, n, 1, st);
     if (!rc) rc = ntt_dispatch(field, d_out, lg, 1, nullptr, st);
     cudaFreeAsync(tmp, st);
     return rc;
 }
 
 int b200_poly_mul_fr_dev(int field, const void *d_a, size_t la, const void *d_b, size_t lb, void *d_out, void *stream) {
-    { int irc = ensure_device_init(); if (irc) return irc; }
-    if (!d_a || !d_b || !d_out) { set_last_error("null pointer"); return B200_EINVAL; }
-    int rc = poly_mul_on_device(field, d_a, la, d_b, lb, d_out, (cudaStream_t)stream);
-    if (rc) return rc;
-    AB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    return 0;
+    return on_stream(stream, [&](cudaStream_t st) {
+        if (!d_a || !d_b || !d_out) { set_last_error("null pointer"); return B200_EINVAL; }
+        return poly_mul_on_device(field, d_a, la, d_b, lb, d_out, st);
+    });
 }
 
 int b200_poly_mul_fr(int field, const uint64_t *a, size_t la, const uint64_t *b, size_t lb, uint64_t *out) {
@@ -627,65 +620,37 @@ int b200_poly_mul_fr(int field, const uint64_t *a, size_t la, const uint64_t *b,
     if (!a || !b || !out) { set_last_error("null pointer"); return B200_EINVAL; }
     const size_t n = b200_poly_mul_size(field, la, lb);
     if (!n) { set_last_error("empty operand or product degree past TWO_ADICITY"); return la && lb ? B200_ETOOLARGE : B200_EINVAL; }
-    cudaStream_t st = 0;
+    HostCall h;
     void *d_a = nullptr, *d_b = nullptr, *d_o = nullptr;
-    AB_CUDA(cudaMallocAsync(&d_a, la * 32, st));
-    AB_CUDA(cudaMallocAsync(&d_b, lb * 32, st));
-    AB_CUDA(cudaMallocAsync(&d_o, n * 32, st));
-    AB_CUDA(cudaMemcpyAsync(d_a, a, la * 32, cudaMemcpyHostToDevice, st));
-    AB_CUDA(cudaMemcpyAsync(d_b, b, lb * 32, cudaMemcpyHostToDevice, st));
-    int rc = poly_mul_on_device(field, d_a, la, d_b, lb, d_o, st);
-    if (!rc) {
-        cudaError_t e = cudaMemcpyAsync(out, d_o, n * 32, cudaMemcpyDeviceToHost, st);
-        if (e != cudaSuccess) rc = cuda_fail(e, "cudaMemcpyAsync D2H", __FILE__, __LINE__);
-    }
-    cudaFreeAsync(d_a, st); cudaFreeAsync(d_b, st); cudaFreeAsync(d_o, st);
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (!rc && e != cudaSuccess) rc = cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
-    return rc;
+    if (int rc = h.begin()) return rc;
+    if (int rc = h.alloc(&d_a, la * 32)) return rc;
+    if (int rc = h.alloc(&d_b, lb * 32)) return rc;
+    if (int rc = h.alloc(&d_o, n * 32)) return rc;
+    if (int rc = h.upload(d_a, a, la * 32)) return rc;
+    if (int rc = h.upload(d_b, b, lb * 32)) return rc;
+    if (int rc = h.wait_uploads()) return rc;
+    if (int rc = poly_mul_on_device(field, d_a, la, d_b, lb, d_o, h.c->st)) return rc;
+    if (int rc = h.download(out, d_o, n * 32)) return rc;
+    return h.sync();
 }
 
 int b200_gen_bases_dev(int curve, uint64_t seed, size_t n, void *d_bases, void *d_b, void *stream) {
-    { int irc = ensure_device_init(); if (irc) return irc; }
-    int rc = gen_bases_dispatch(curve, seed, n, d_bases, d_b, (cudaStream_t)stream);
-    if (rc) return rc;
-    AB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    return 0;
+    return on_stream(stream, [&](cudaStream_t st) { return gen_bases_dispatch(curve, seed, n, d_bases, d_b, st); });
 }
 int b200_gen_scalars_dev(int field, uint64_t seed, size_t n, void *d_scalars, void *stream) {
-    { int irc = ensure_device_init(); if (irc) return irc; }
-    int rc = gen_scalars_dispatch(field, seed, n, d_scalars, (cudaStream_t)stream);
-    if (rc) return rc;
-    AB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    return 0;
+    return on_stream(stream, [&](cudaStream_t st) { return gen_scalars_dispatch(field, seed, n, d_scalars, st); });
 }
 int b200_g1_batch_mul_dev(int curve, const uint64_t *base_xy, const void *d_scalars, size_t n, void *d_out_xy, void *stream) {
-    { int irc = ensure_device_init(); if (irc) return irc; }
-    int rc = batch_mul_dispatch(curve, base_xy, d_scalars, n, d_out_xy, (cudaStream_t)stream);
-    if (rc) return rc;
-    AB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    return 0;
+    return on_stream(stream, [&](cudaStream_t st) { return batch_mul_dispatch(curve, base_xy, d_scalars, n, d_out_xy, st); });
 }
 int b200_g1_normalize_batch_dev(int curve, const void *d_xyz, size_t n, void *d_out_xy, void *stream) {
-    { int irc = ensure_device_init(); if (irc) return irc; }
-    int rc = normalize_batch_dispatch(curve, d_xyz, n, d_out_xy, (cudaStream_t)stream);
-    if (rc) return rc;
-    AB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    return 0;
+    return on_stream(stream, [&](cudaStream_t st) { return normalize_batch_dispatch(curve, d_xyz, n, d_out_xy, st); });
 }
 int b200_fp_op_dev(int field, int op, const void *d_a, const void *d_b, void *d_out, size_t n, int reps, void *stream) {
-    { int irc = ensure_device_init(); if (irc) return irc; }
-    int rc = fp_op_dispatch(field, op, d_a, d_b, d_out, n, reps, (cudaStream_t)stream);
-    if (rc) return rc;
-    AB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    return 0;
+    return on_stream(stream, [&](cudaStream_t st) { return fp_op_dispatch(field, op, d_a, d_b, d_out, n, reps, st); });
 }
 int b200_ec_op_dev(int curve, int op, const void *d_a, const void *d_b, void *d_out, size_t n, void *stream) {
-    { int irc = ensure_device_init(); if (irc) return irc; }
-    int rc = ec_op_dispatch(curve, op, d_a, d_b, d_out, n, (cudaStream_t)stream);
-    if (rc) return rc;
-    AB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    return 0;
+    return on_stream(stream, [&](cudaStream_t st) { return ec_op_dispatch(curve, op, d_a, d_b, d_out, n, st); });
 }
 int b200_msm_last_timings(float *ms7, int *c, int *windows, unsigned long long *bucket_adds) { return msm_last_timings(ms7, c, windows, bucket_adds); }
 

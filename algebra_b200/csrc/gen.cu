@@ -7,6 +7,7 @@
 #include <mutex>
 
 #include "common.cuh"
+#include "host_api.h"
 #include "ec.cuh"
 
 namespace ab200 {

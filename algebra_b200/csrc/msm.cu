@@ -26,6 +26,7 @@
 #include <memory>
 #include <vector>
 
+#include "host_api.h"
 #include "msm_common.cuh"
 
 namespace ab200 {
@@ -258,6 +259,10 @@ static int scalar_kind_bits(int kind, int field_bits) {
         default: return field_bits;  // Fr::MODULUS_BIT_SIZE (variable_base/mod.rs:451)
     }
 }
+int check_scalar_kind(int kind) {
+    if (kind < B200_SCALARS_FR_MONT || kind > B200_SCALARS_U64) { set_last_error("unknown scalar kind"); return B200_EINVAL; }
+    return 0;
+}
 size_t scalar_kind_bytes(int kind) {
     switch (kind) {
         case B200_SCALARS_U8: return 1;
@@ -323,19 +328,6 @@ static int sm_count() {
     }
     return cached;
 }
-
-struct MsmSessionBase {
-    virtual ~MsmSessionBase() {}
-    // n_total: expected total number of pairs (window choice); max_chunk: largest chunk handed to add_chunk
-    virtual int begin(size_t n_total, size_t max_chunk, int kind, cudaStream_t st) = 0;
-    // digit-sort + accumulate one chunk into the session's buckets; `ready` (may be null) is waited on first.  Asynchronous.
-    virtual int add_chunk(const void *d_bases, const void *d_scalars, size_t nk, cudaEvent_t ready) = 0;
-    // bucket reduction + window combine -> d_out (3 coordinates, Jacobian).  Asynchronous on the session's stream.
-    virtual int finish(void *d_out) = 0;
-    // after the stream has been synchronised: fold the per-phase events into the thread's "last timings"
-    virtual int collect_timings() = 0;
-    virtual int coord_words() const = 0;   // 32-bit words per coordinate (12 / 8 / 24)
-};
 
 template <class C> struct MsmSession final : MsmSessionBase {
     using F = typename C::F;
@@ -627,13 +619,24 @@ MsmSessionBase *msm_session_create(int curve) {
     }
     return nullptr;
 }
-int msm_coord_words(int curve) {
+const CurveInfo *curve_info(int curve) {
+    static const CurveInfo bls = {CurveBls::F::L, CurveBls::SCALAR_BITS, B200_FIELD_BLS12_381_FR},
+                           bn = {CurveBn::F::L, CurveBn::SCALAR_BITS, B200_FIELD_BN254_FR},
+                           g2 = {CurveBlsG2::F::L, CurveBlsG2::SCALAR_BITS, B200_FIELD_BLS12_381_FR};
     switch (curve) {
-        case B200_CURVE_BLS12_381: return 12;
-        case B200_CURVE_BN254: return 8;
-        case B200_CURVE_BLS12_381_G2: return 24;
+        case B200_CURVE_BLS12_381: return &bls;
+        case B200_CURVE_BN254: return &bn;
+        case B200_CURVE_BLS12_381_G2: return &g2;
     }
-    return 0;
+    return nullptr;
+}
+const FieldInfo *field_info(int field) {
+    static const FieldInfo bls = {BlsFr::TWO_ADICITY, 1}, bn = {BnFr::TWO_ADICITY, 3};
+    switch (field) {
+        case B200_FIELD_BLS12_381_FR: return &bls;
+        case B200_FIELD_BN254_FR: return &bn;
+    }
+    return nullptr;
 }
 static uint32_t curve_one_limb(int curve, int i) {   // Montgomery ONE of the coordinate field, 32-bit word i
     switch (curve) {
@@ -644,7 +647,7 @@ static uint32_t curve_one_limb(int curve, int i) {   // Montgomery ONE of the co
 }
 // Projective::zero() = (1,1,0) (group.rs:142-158) as 3 coordinates of L words, written as u64 limbs
 void msm_write_zero(int curve, uint64_t *out_xyz) {
-    const int L = msm_coord_words(curve);
+    const int L = curve_info(curve)->coord_words;
     for (int i = 0; i < 3 * L / 2; i++) out_xyz[i] = 0;
     for (int k = 0; k < 2; k++)
         for (int i = 0; i < L; i++) out_xyz[(k * L + i) / 2] |= (uint64_t)curve_one_limb(curve, i) << (32 * ((k * L + i) & 1));
@@ -655,10 +658,10 @@ void msm_write_zero(int curve, uint64_t *out_xyz) {
 // bucket reduction and window combine run once at the end.
 int msm_dispatch(int curve, int kind, const void *d_bases, const void *d_scalars, size_t n, uint64_t *out_xyz_host, cudaStream_t st, int K,
                  const size_t *chunk_off, const cudaEvent_t *ready) {
-    if (kind < B200_SCALARS_FR_MONT || kind > B200_SCALARS_U64) { set_last_error("unknown scalar kind"); return B200_EINVAL; }
+    if (int rc = check_scalar_kind(kind)) return rc;
     if (!out_xyz_host || (n && (!d_bases || !d_scalars))) { set_last_error("null pointer"); return B200_EINVAL; }
-    const int L = msm_coord_words(curve);
-    if (!L) { set_last_error("unknown curve id"); return B200_EINVAL; }
+    const CurveInfo *ci = curve_info(curve);
+    if (!ci) { set_last_error("unknown curve id"); return B200_EINVAL; }
     if (n == 0) { msm_write_zero(curve, out_xyz_host); return 0; }
     if (n >= ((size_t)1 << 31)) { set_last_error("n must be < 2^31"); return B200_ETOOLARGE; }
     // device-resident inputs too large for one 31-bit entry index space (n * windows >= 2^31): split into equal chunks
@@ -679,23 +682,28 @@ int msm_dispatch(int curve, int kind, const void *d_bases, const void *d_scalars
     const size_t sb = scalar_kind_bytes(kind);
     int rc = s->begin(n, max_chunk, kind, st);
     for (int k = 0; k < K && !rc; k++)
-        rc = s->add_chunk((const char *)d_bases + chunk_off[k] * (size_t)(2 * L * 4), (const char *)d_scalars + chunk_off[k] * sb,
+        rc = s->add_chunk((const char *)d_bases + chunk_off[k] * (size_t)(2 * ci->coord_words * 4), (const char *)d_scalars + chunk_off[k] * sb,
                           chunk_off[k + 1] - chunk_off[k], ready ? ready[k] : nullptr);
-    uint32_t *d_out = nullptr;
+    if (rc) { cudaStreamSynchronize(st); return rc; }   // nothing of this call is in flight when it returns
+    return msm_session_result(*s, out_xyz_host, st);   // ~MsmSession frees the scratch and the events
+}
+
+int msm_session_result(MsmSessionBase &s, uint64_t *out_xyz, cudaStream_t st) {
+    const size_t bytes = (size_t)3 * s.coord_words() * 4;
+    void *d_out = nullptr;
+    int rc = 0;
+    cudaError_t e = cudaMallocAsync(&d_out, bytes, st);
+    if (e != cudaSuccess) rc = cuda_fail(e, "cudaMallocAsync", __FILE__, __LINE__);
+    if (!rc) rc = s.finish(d_out);
     if (!rc) {
-        cudaError_t e = cudaMallocAsync(&d_out, 3 * L * 4, st);
-        if (e != cudaSuccess) rc = cuda_fail(e, "cudaMallocAsync", __FILE__, __LINE__);
-    }
-    if (!rc) rc = s->finish(d_out);
-    if (!rc) {
-        cudaError_t e = cudaMemcpyAsync(out_xyz_host, d_out, 3 * L * 4, cudaMemcpyDeviceToHost, st);
+        e = cudaMemcpyAsync(out_xyz, d_out, bytes, cudaMemcpyDeviceToHost, st);
         if (e != cudaSuccess) rc = cuda_fail(e, "cudaMemcpyAsync D2H", __FILE__, __LINE__);
     }
     if (d_out) cudaFreeAsync(d_out, st);
-    cudaError_t e = cudaStreamSynchronize(st);   // also on the error paths: nothing of this call is in flight when it returns
+    e = cudaStreamSynchronize(st);   // also on the error paths: nothing of the session's work is in flight when it returns
     if (!rc && e != cudaSuccess) rc = cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
-    if (!rc) rc = s->collect_timings();
-    return rc;   // ~MsmSession frees the scratch and the events
+    if (!rc) rc = s.collect_timings();
+    return rc;
 }
 
 int msm_last_timings(float *ms7, int *c, int *windows, unsigned long long *bucket_adds) {
@@ -706,26 +714,16 @@ int msm_last_timings(float *ms7, int *c, int *windows, unsigned long long *bucke
     return 0;
 }
 
-int g1_sum_dispatch(int curve, const uint64_t *pts_host, size_t k, uint64_t *out_host, bool to_affine) {
-    const int L = msm_coord_words(curve);
-    if (!L) { set_last_error("unknown curve id"); return B200_EINVAL; }
-    if (!pts_host || !out_host) { set_last_error("null pointer"); return B200_EINVAL; }
-    const size_t in_words = k * 3 * L, out_words = to_affine ? k * 2 * L : 3 * L;
-    cudaStream_t st = 0;
-    StreamArena arena;
-    arena.st = st;
-    uint32_t *d_in = nullptr, *d_out = nullptr;
-    if (int rc = arena.alloc(&d_in, std::max<size_t>(in_words, 1) * 4)) return rc;
-    if (int rc = arena.alloc(&d_out, std::max<size_t>(out_words, 1) * 4)) return rc;
-    AB_CUDA(cudaMemcpyAsync(d_in, pts_host, in_words * 4, cudaMemcpyHostToDevice, st));
-    int rc;
-    if (curve == B200_CURVE_BLS12_381) rc = MsmRedLaunch<CurveBls>::sum_or_affine(to_affine, d_in, k, d_out, st);
-    else if (curve == B200_CURVE_BN254) rc = MsmRedLaunch<CurveBn>::sum_or_affine(to_affine, d_in, k, d_out, st);
-    else rc = MsmRedLaunch<CurveBlsG2>::sum_or_affine(to_affine, d_in, k, d_out, st);
-    if (rc) return rc;
-    AB_CUDA(cudaMemcpyAsync(out_host, d_out, out_words * 4, cudaMemcpyDeviceToHost, st));
-    AB_CUDA(cudaStreamSynchronize(st));
-    return 0;
+int g1_sum(int curve, const void *d_pts, size_t k, void *d_out, bool to_affine, cudaStream_t st) {
+    const uint32_t *in = (const uint32_t *)d_pts;
+    uint32_t *out = (uint32_t *)d_out;
+    switch (curve) {
+        case B200_CURVE_BLS12_381: return MsmRedLaunch<CurveBls>::sum_or_affine(to_affine, in, k, out, st);
+        case B200_CURVE_BN254: return MsmRedLaunch<CurveBn>::sum_or_affine(to_affine, in, k, out, st);
+        case B200_CURVE_BLS12_381_G2: return MsmRedLaunch<CurveBlsG2>::sum_or_affine(to_affine, in, k, out, st);
+    }
+    set_last_error("unknown curve id");
+    return B200_EINVAL;
 }
 
 }  // namespace ab200

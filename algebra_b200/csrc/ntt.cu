@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "host_api.h"
 
 namespace ab200 {
 

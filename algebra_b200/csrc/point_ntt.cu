@@ -15,6 +15,7 @@
 // Work: (n/2)·k butterflies, of which n - 1 have twiddle 1 (no ladder); one ladder per element for each scale pass.
 #include "common.cuh"
 #include "ec.cuh"
+#include "host_api.h"
 
 namespace ab200 {
 
@@ -230,14 +231,12 @@ int point_ntt_check(int curve, const void *points, uint32_t log_n) {
         return B200_EINVAL;
     }
     if (!points) { set_last_error("null points pointer"); return B200_EINVAL; }
-    if (log_n > (uint32_t)(curve == B200_CURVE_BLS12_381 ? BlsFr::TWO_ADICITY : BnFr::TWO_ADICITY)) {
+    if (log_n > (uint32_t)field_info(curve_info(curve)->scalar_field)->two_adicity) {
         set_last_error("log_n exceeds TWO_ADICITY (Radix2EvaluationDomain::new would return None)");
         return B200_ETOOLARGE;
     }
     return 0;
 }
-
-int point_ntt_coord_words(int curve) { return curve == B200_CURVE_BLS12_381 ? BlsFq::L : BnFq::L; }
 
 int point_ntt_dispatch(int curve, void *d_points, uint32_t log_n, int inverse, const uint64_t *coset, cudaStream_t st) {
     if (int rc = point_ntt_check(curve, d_points, log_n)) return rc;

@@ -1,6 +1,7 @@
 // prims.cu — element-wise kernels over the device arithmetic headers (1 thread per element): the parity surface for
 // fp.cuh / ec.cuh on the real GPU and the field micro-benchmark (cf. bench-templates/src/macros/field.rs:69-155).
 #include "common.cuh"
+#include "host_api.h"
 #include "ec.cuh"
 
 namespace ab200 {

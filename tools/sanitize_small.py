@@ -10,6 +10,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import algebra_b200 as ab
 from algebra_b200 import _lib
 from algebra_b200 import variable_base as VB
+from algebra_b200.params import CURVES
 
 L = _lib.lib()
 st = torch.cuda.current_stream().cuda_stream
@@ -39,6 +40,13 @@ for cid, N in ((0, 6), (1, 4), (2, 12)):
     for lo in range(0, n, 700):
         stream.push(hb[lo:lo + 700], hs[lo:lo + 700])
     assert (ab.into_affine(cid, stream.finish()) == ref).all()
+    # host-buffer entry points: leased context, staged uploads, download on the compute stream
+    assert (ab.into_affine(cid, ab.msm_multi(cid, hb, hs, 1)) == ref).all()
+    h = ab.bases_upload(cid, hb)
+    assert (ab.into_affine(cid, ab.msm_with_bases(h, hs)) == ref).all()
+    ab.bases_free(h)
+    halves = np.stack([ab.msm(cid, hb[:1000], hs[:1000]), ab.msm(cid, hb[1000:], hs[1000:])])
+    assert (ab.into_affine(cid, ab.sum_points(cid, halves)) == ref).all()
     if cid == 2:
         continue                                                  # the remaining calls are G1 / scalar-field only
     same = torch.zeros_like(d_s)
@@ -59,7 +67,19 @@ for cid, N in ((0, 6), (1, 4), (2, 12)):
     co.fft_in_place(x)
     co.ifft_in_place(x)
     assert torch.equal(x, x0)
-    ab.poly_mul(cid, x[:300], x[300:500])
+    short = x0[:1000].cpu().numpy().view(np.uint64)                # pageable and shorter than the domain: padded on the device
+    padded = torch.zeros_like(x0)
+    padded[:1000] = x0[:1000]
+    assert (dom.fft(short) == dom.fft(padded).cpu().numpy().view(np.uint64)).all()
+    prod = ab.poly_mul(cid, x[:300], x[300:500])
+    hx = x.cpu().numpy().view(np.uint64)
+    assert (ab.poly_mul(cid, hx[:300], hx[300:500]) == prod.cpu().numpy().view(np.uint64)).all()
+    jac = np.zeros((16, 3 * N), dtype=np.uint64)                  # bases with z = 1 (Montgomery form)
+    jac[:, :2 * N] = hb[:16]
+    jac[:, 2 * N:] = CURVES[cid].fq.to_limbs(1)
+    dom_p = ab.Radix2EvaluationDomain.new(cid, 16)
+    want = dom_p.fft(torch.from_numpy(jac.view(np.int64)).cuda(), curve=cid).cpu().numpy().view(np.uint64)
+    assert (dom_p.fft(jac, curve=cid) == want).all()
     dom16 = ab.Radix2EvaluationDomain.new(cid, 1 << 16)            # two passes of 256 and 256
     y = torch.empty((1 << 16, 4), dtype=torch.int64, device="cuda")
     _lib.check(L.b200_gen_scalars_dev(cid, 10, 1 << 16, y.data_ptr(), st))
